@@ -1,5 +1,5 @@
 #!/usr/bin/env python
-"""bench.py -- rays/s of a 512x512 avatar render (BASELINE.json metric) on N B200s.
+"""bench.py -- rays/s of a 512x512 avatar render (BASELINE.json metric) on N H100s.
 
 A "step" is one complete frame of the reference's `render_image_fast` (DNeRF.py:72-97) on the synthetic
 PeopleSnapshot-shaped scene (SURVEY.md §8d): SMPL forward -> bone transforms -> skinning-transform field ->
@@ -10,6 +10,8 @@ hash-grid / MLP / compositing kernel.
   e2e   : the same frame through the public API with HOST buffers: pinned rays + pose -> device, render, RGBA -> host.
   --impl reference : the CPU oracle (C port of the reference's kernels + numpy host loop, all host threads) on the same
                      frame -- the reference's own GPU path needs tiny-cuda-nn, which cannot be built (BASELINE.md §2).
+  --dump-outputs DIR : after the timed steps, writes the RGB / depth / alpha / sample-count images of the last timed
+                     frame as DIR/<name>.npy (float32); inputs are seeded, so equal arguments give equal inputs.
 N > 1: one process per GPU (torchrun), each rank renders whole frames of different poses; no data-path collective
 ("scaling": "weak").
 """
@@ -46,11 +48,13 @@ def parse():
     ap.add_argument("--train-rays-per-warp", type=int, default=0)
     ap.add_argument("--render-warps", type=int, default=0, help="warps per CTA of the fused renderer (12)")
     ap.add_argument("--query-warps", type=int, default=0, help="warps per CTA of the point-query kernel (12 / 16 / 20)")
+    ap.add_argument("--dump-outputs", metavar="DIR", default=None,
+                    help="write what the last timed step computed as DIR/<name>.npy (float32)")
     return ap.parse_args()
 
 
 # ------------------------------------------------------------------------------------------------
-# clocks sampler (B200_PROFILING.md recipe)
+# clocks sampler
 # ------------------------------------------------------------------------------------------------
 class ClockSampler:
     Q = "index,clocks.sm,clocks.max.sm,power.draw,clocks_event_reasons.hw_slowdown,clocks_event_reasons.hw_thermal_slowdown,clocks_event_reasons.sw_thermal_slowdown,clocks_event_reasons.sw_power_cap"
@@ -269,7 +273,7 @@ def bench_ref_structure(model, batch, device, iters=5):
         ms = float(np.median(t_all))
         return {"ms_per_frame": ms, "rays_per_s": N_RAYS / (ms * 1e-3), "ms_render_test_only": float(np.median(t_march)),
                 "alpha_sum": float(out["alpha"].sum().item()),
-                "what": "reference kernels (raymarcher.cu, fuse_cuda_kernel_fast.cu, filter.cu, precompute.cu built for sm_100) + "
+                "what": "reference kernels (raymarcher.cu, fuse_cuda_kernel_fast.cu, filter.cu, precompute.cu built for sm_90) + "
                         "reference host loop; tiny-cuda-nn replaced by ia_ngp_forward; SMPL forward excluded"}
     except Exception as e:  # the checker must never take the bench down
         return {"unavailable": f"{type(e).__name__}: {e}"}
@@ -302,7 +306,7 @@ def bench_train(model, batch, device, rank, world, flush, steps=40, warmup=25, u
         b[k] = batch[k][:, pick].contiguous()
     a = alpha_gt[pick][None]
     model.configure_parallel(world)
-    if train_rays_per_warp:  # sweeps (scripts/train_scaling.py) override the tile size configure_parallel picked
+    if train_rays_per_warp:  # sweeps override the tile size configure_parallel picked
         from instantavatar_b200 import ops as _ops
         _ops.set_option("train_rays_per_warp", train_rays_per_warp)
     model.global_step = 2000  # steady state: no density noise, grid refresh uses the previous field as `valid`
@@ -537,6 +541,13 @@ def bench_optimizer_step(model, device, world, iters=30):
     return {"ms": float(ms.item()), "path": "peer" if getattr(opt, "_peer", None) else "nccl"}
 
 
+def dump_outputs(out_dir: str, arrays: dict):
+    """the frame a caller of the timed path receives, as float32 .npy files (512x512: 9 MB in all)"""
+    os.makedirs(out_dir, exist_ok=True)
+    for name, t in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), t.detach().float().cpu().numpy())
+
+
 def run_ours(args):
     import torch
     import torch.distributed as dist
@@ -547,6 +558,7 @@ def run_ours(args):
     local = int(os.environ.get("LOCAL_RANK", "0"))
     torch.cuda.set_device(local)
     device = torch.device("cuda", local)
+    torch.manual_seed(0)  # the occupancy-grid jitter drawn inside the frame: identical inputs from run to run
     if world > 1:
         dist.init_process_group("nccl", device_id=device)
     sampler = ClockSampler(local)
@@ -567,7 +579,7 @@ def run_ours(args):
     h2d_bytes = sum(v.numel() * v.element_size() for v in pinned.values())
     out_host = torch.empty((N_RAYS, 4), dtype=torch.float32).pin_memory()
     d2h_bytes = out_host.numel() * 4
-    flush = torch.empty(192 * 1024 * 1024, dtype=torch.uint8, device=device)  # > 126 MB L2
+    flush = torch.empty(128 * 1024 * 1024, dtype=torch.uint8, device=device)  # > 50 MB L2 of an H100
 
     from instantavatar_b200.graphs import GraphedFrame
     use_graph = not args.no_graph
@@ -597,22 +609,26 @@ def run_ours(args):
             fn()
         barrier()
         ev = [(torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)) for _ in range(steps)]
+        out = None
         for a, b in ev:
             flush.zero_()  # L2 flush between timed iterations (outside the event bracket)
-            a.record(); fn(); b.record()
+            a.record(); out = fn(); b.record()
         barrier()
         ms = [a.elapsed_time(b) for a, b in ev]
         tot = torch.tensor([sum(ms)], device=device, dtype=torch.float64)
         if world > 1:
             dist.all_reduce(tot, op=dist.ReduceOp.MAX)
-        return float(tot.item()), ms
+        return float(tot.item()), ms, out
 
     # nvidia-smi needs a few hundred ms before its first row: the sampler was started before the model was built
     t_load0 = time.monotonic()
     _lib.LAUNCHES = 0
-    total_ms, per = timed(step_resident, args.steps, max(args.warmup, 3))
+    total_ms, per, last = timed(step_resident, args.steps, max(args.warmup, 3))
     launches = getattr(_lib, "LAUNCHES", 0)
-    e2e_ms, _ = timed(step_e2e, args.steps, 3)
+    if args.dump_outputs and rank == 0:
+        # copied before the e2e leg replays the same graph into the same output buffers
+        dump_outputs(args.dump_outputs, dict(zip(("rgb", "depth", "alpha", "counter"), last)))
+    e2e_ms, _, _ = timed(step_e2e, args.steps, 3)
     t_load1 = time.monotonic()
     clocks = None
     if rank == 0:
@@ -688,10 +704,10 @@ def run_ours(args):
         peaks = json.load(open(os.path.join(ROOT, "MEASURED_PEAKS.json")))
     except Exception:
         pass
-    hbm_peak, peak_src = (peaks.get("hbm_gbs"), "measured") if peaks.get("hbm_gbs") else (6650.0, "fallback")
+    hbm_peak, peak_src = (peaks.get("hbm_gbs"), "measured") if peaks.get("hbm_gbs") else (3350.0, "H100 SXM data sheet")
     # Sectors the kernels REQUEST (kernel counters; exact-zero footprints and early-out solves issue nothing and are not
     # counted): 12 x 32 B per field footprint that loaded, one sector per hash-table load a lane issues (128 per network
-    # evaluation: 16 levels x 8 corners).  The ceiling is the same shape in isolation (lane = footprint, 12 LDG.E.256, next
+    # evaluation: 16 levels x 8 corners).  The ceiling is the same shape in isolation (lane = footprint, 12 sectors, next
     # address data-dependent) measured in this run: frac = requested sectors / s over that.
     q_sect = qst["field_loads"] * 12 + qst["hash_loads"]
     r_sect = st["field_loads"] * 12 + st["hash_loads"]
@@ -739,7 +755,7 @@ def run_ours(args):
                      "compulsory_dram_bytes": field_bytes + table_bytes,
                      "render_kernel": "render_fwd_kernel", "render_achieved": r_gbs, "render_frac": r_gbs / ceil_gbs,
                      "render_kernel_ms": k_ms, "render_sectors_requested": r_sect,
-                     "note": "gather-bound on L2-resident tables (76 MB): achieved = 32 B x sectors the kernel requests / CUDA-event time; peak = the same access shape in isolation (L1 data pipe + L2), not HBM; DRAM traffic is the compulsory table read (ncu captures in profiles/)"},
+                     "note": "gather-bound on L2-resident tables (76 MB): achieved = 32 B x sectors the kernel requests / CUDA-event time; peak = the same access shape in isolation (L1 data pipe + L2), not HBM; DRAM traffic is the compulsory table read"},
         "work_per_frame": st, "work_per_occupancy_init": qst,
         "train": train, "grad_collective": comm, "frame_sharded": sharded, "multi_gpu_checks": checks,
         "next_rows": next_rows, "ref_structure": ref_struct,

@@ -1,5 +1,5 @@
 /*
- * ia_b200.h -- C ABI of libia_b200.so, the B200 (sm_100a) implementation of InstantAvatar's per-ray hot
+ * ia_b200.h -- C ABI of libia_b200.so, the H100 (sm_90a) implementation of InstantAvatar's per-ray hot
  * path.  Plain pointers and sizes only; every pointer is a DEVICE pointer unless marked [host]; all
  * buffers are owned by the caller (the library never allocates, frees or retains pointers, and never
  * synchronises the device).  Every entry point enqueues work on `stream` and returns 0, or a negative
@@ -271,7 +271,7 @@ int ia_train_fwd(const IaScene* scene /*[host]*/, const float* rays_o, const flo
  * steps become consecutive slots, their jittered posed points are appended to a device-side sample list; (2) the point-query
  * kernel over that list, every 32-sample batch an independent work item of all resident warps; (3) per-ray compositing.
  * ia_train_fwd walks a tile's samples inside one warp, so its time is the heaviest tile's critical path (it does not shrink
- * below ~0.36 ms however few rays a step has); this form scales with the number of samples.  workspace:
+ * however few rays a step has); this form scales with the number of samples.  workspace:
  * ia_train_fwd_workspace_bytes(n_rays) (256 + 4 * n_rays * 256). */
 size_t ia_train_fwd_workspace_bytes(int n_rays);
 int ia_train_fwd_split(const IaScene* scene /*[host]*/, const float* rays_o, const float* rays_d, const float* near,

@@ -1,6 +1,6 @@
 """ctypes binding of libia_b200.so (include/ia_b200.h).
 
-There is no CPU fallback: importing this module without the compiled sm_100a library raises, and every
+There is no CPU fallback: importing this module without the compiled sm_90a library raises, and every
 entry point requires CUDA tensors.  PyTorch is used only for device memory and streams.
 """
 from __future__ import annotations
@@ -11,7 +11,7 @@ import os
 import torch
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# IA_B200_LIB: an alternative build of the same sources (experiments only, e.g. scripts/build_variant.sh -fmad=true)
+# IA_B200_LIB: an alternative build of the same sources (experiments only, e.g. one compiled with -fmad=true)
 LIB_PATH = os.environ.get("IA_B200_LIB") or os.path.join(_HERE, "libia_b200.so")
 
 IA_MLP_HALFS = 22144

@@ -1,5 +1,5 @@
-// ia_kernels.cu -- sm_100a kernels + the extern "C" boundary of libia_b200.so (include/ia_b200.h).
-// Build: nvcc -gencode arch=compute_100a,code=sm_100a -fmad=false -lineinfo -O3 -std=c++17 (see build.py).
+// ia_kernels.cu -- sm_90a kernels + the extern "C" boundary of libia_b200.so (include/ia_b200.h).
+// Build: nvcc -gencode arch=compute_90a,code=sm_90a -fmad=false -lineinfo -O3 -std=c++17 (see __graft_entry__.py).
 #include <math.h>
 #include <stdio.h>
 #include <string.h>
@@ -874,8 +874,8 @@ int ia_set_option(const char* name, int value) {
         return IA_OK;
     }
     if (!strcmp(name, "render_warps")) {
-        // 12 only: the 16-warp build (128 registers) was measured slower (profiles/sweep_warps_r2.jsonl) and does not fit
-        // next to the staged hash level; the name stays so that old sweep scripts fail loudly on other values
+        // 12 only: the 16-warp build (128 registers) does not fit next to the staged hash level; the name stays so that
+        // callers passing other values fail loudly
         IA_REQUIRE(value == 12);
         return IA_OK;
     }
@@ -1046,7 +1046,7 @@ static int render_fwd_impl(const IaScene* scene, const float* rays_o, const floa
     int* ws_cost = reinterpret_cast<int*>(reinterpret_cast<char*>(workspace) + 256);
     int* ws_order = ws_cost + (n_rays + 1);
     const int rpw = g_render_rays;
-    // (a 16-warp renderer was measured slower, profiles/sweep_warps_r2.jsonl, and no longer fits next to the staged hash level)
+    // (a 16-warp renderer no longer fits next to the staged hash level)
     switch (rpw) {
         case 32: rc = launch_render<12, 32>(a, plan, ws_cost, ws_order, st); break;
         case 16: rc = launch_render<12, 16>(a, plan, ws_cost, ws_order, st); break;
@@ -1134,8 +1134,7 @@ static int occupancy_query_impl(const IaScene* scene, const float* jitter, const
     a.n_dev = nullptr; a.index = nullptr;
     // several lanes per point ("occupancy_lanes_per_point") were measured and do NOT pay here, unlike in the training list
     // query: 98 % of the grid points are empty space whose solves end after one or two gathers, so splitting a point's 13
-    // solves over lanes shortens nothing and idles the helper lanes in every later stage (1/8 shard: 0.295 -> 0.297 ms
-    // with 2 lanes, 0.50 ms with 4; whole grid 1.60 -> 1.80 / 3.39 ms; profiles/query_schedule_r2.jsonl).  Default 1.
+    // solves over lanes shortens nothing and idles the helper lanes in every later stage.  Default 1.
     a.lanes_per_sample = g_occ_lanes ? g_occ_lanes : 1;
     if (batch_order || batch_cost || 32 / a.lanes_per_sample < passes) a.lanes_per_sample = 1;
     IA_REQUIRE(!batch_order || (workspace && n_order >= 0));

@@ -2,13 +2,12 @@
 //
 // deform_query_kernel / render_fwd_kernel / train_fwd_kernel spend their memory time in one access shape: every lane
 // gathers its own trilinear footprint of the skinning-transform field -- 4 x-pair records of 96 bytes = 12 sectors,
-// 12 x LDG.E.256 -- from an L2-resident 50 MB table, and the next address depends on the loaded data (a Broyden
+// 24 x LDG.E.128 -- from a 50 MB table, and the next address depends on the loaded data (a Broyden
 // iterate).  This kernel issues exactly that shape and nothing else (no solver arithmetic beyond the 96 FMAs that
 // consume the loads), at the fused kernels' residency (one CTA of `warps` warps per SM, persistent), so
 //     sectors requested / time  =  what the L1 data pipe + L2 deliver for this shape on this GPU.
 // `coherent` = 1 keeps the lanes of a warp inside a 10 x 3 x 3 voxel neighbourhood as a batch of the occupancy query does
-// (6 neighbouring grid cells x 5 jitters); 0 = independent footprints per lane.  scripts/gather_ceiling.cu sweeps more
-// fetch shapes (cooperative lines, TMA-engine bulk copies, tensor-map boxes); this is the one the kernels use.
+// (6 neighbouring grid cells x 5 jitters); 0 = independent footprints per lane.
 #include "ia_device.cuh"
 #include "ia_host.h"
 
@@ -45,7 +44,7 @@ __global__ void __launch_bounds__(kWarps * 32, 1) gather_ceiling_kernel(const fl
 #pragma unroll
         for (int k = 0; k < 4; k++) {
             const float* p = table + (size_t)rec[k] * kVoxelFloats;
-            const F8 A = ldg256(p), B = ldg256(p + 8), C3 = ldg256(p + 16);
+            const F8 A = ldg_sector(p), B = ldg_sector(p + 8), C3 = ldg_sector(p + 16);
 #pragma unroll
             for (int c = 0; c < 8; c++) acc[c] = __fmaf_rn(A.v[c], w0, acc[c]);
 #pragma unroll

@@ -213,7 +213,7 @@ __global__ void __launch_bounds__(kWarps * 32, 1) train_fwd_kernel(const __grid_
 // ================================================================================================
 // split training forward: march -> sample list -> point query over the list -> per-ray compositing.
 // The fused kernel above walks a tile's samples 32 at a time inside ONE warp, so a step takes as long as its heaviest
-// tile (390 / 385 / 363 us at 4096 / 2048 / 512 rays: it does not shrink with the ray count).  Here every 32-sample batch
+// tile (it does not shrink with the ray count).  Here every 32-sample batch
 // of the step is an independent work item of the point-query kernel (ia_kernels.cu), spread over all resident warps.
 // Arithmetic per sample and per ray is the fused kernel's, operation for operation (same results, bit for bit).
 // ================================================================================================
@@ -299,8 +299,7 @@ struct TrainCompositeArgs {
 
 // one warp per ray: 32 slots are loaded at once (coalesced) and their alphas computed in parallel; the transmittance and
 // the five sums then advance slot by slot in the fused kernel's order (operands broadcast by shuffle), so the results are
-// bit-identical.  (The first version, one thread per ray with 8-slot staging, cost 20 us at any ray count: a 256-slot ray
-// is 32 dependent load round trips.)
+// bit-identical.  (One thread per ray with 8-slot staging would make a 256-slot ray 32 dependent load round trips.)
 __global__ void __launch_bounds__(256) train_composite_kernel(TrainCompositeArgs a) {
     const int lane = threadIdx.x & 31;
     const int ray = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -364,8 +363,8 @@ struct CompBwdArgs {
 
 // One warp per ray: 32 slots are loaded at once (coalesced) and everything that does not depend on the transmittance
 // recurrence (exp, alpha, the upstream dot products) is computed in parallel; the recurrence itself runs slot by slot in the
-// original order with operands broadcast by shuffle, each lane keeping the values of its own slot.  (The thread-per-ray
-// version took ~50 us at any ray count: a 256-slot ray is 2 x 32 dependent load round trips.)  Same list layout as before:
+// original order with operands broadcast by shuffle, each lane keeping the values of its own slot.  (Thread per ray, a
+// 256-slot ray would be 2 x 32 dependent load round trips.)  Same list layout as before:
 // a ray's samples occupy one contiguous block in slot order.
 __global__ void __launch_bounds__(256) composite_bwd_kernel(CompBwdArgs a) {
     const int lane = threadIdx.x & 31;
@@ -1078,9 +1077,7 @@ __global__ void adam_prepare_kernel(float* state, float inv_world, const float* 
 // HBM-bound streaming pass: 34 bytes per parameter (g, p, m, v read; g, p, m, v written; fp16 image written).  All four
 // loads are issued up front -- they do not wait for the overflow flag or the step state, which sit in shared memory -- and
 // every access carries the evict-first hint (ld.global.cs / st.global.cs): nothing here is reused, and without the hint
-// the 443 MB stream thrashes the L2 that it shares with its own write-backs.  Measured on the 13 M-parameter vector
-// (scripts/adam_variants.cu, profiles/adam_variants_r2.jsonl): 0.203 ms (2.2 TB/s) for the round-1 shape -> 0.075 ms
-// (5.9 TB/s, 0.91 of the measured copy bandwidth).
+// the 443 MB stream thrashes the L2 that it shares with its own write-backs.
 __global__ void __launch_bounds__(256) adam_dev_kernel(float4* __restrict__ p, float4* __restrict__ g, float4* __restrict__ m,
                                                         float4* __restrict__ v, long n4, const float* __restrict__ state,
                                                         const float* __restrict__ found_inf, uint2* __restrict__ half_out,
@@ -1718,8 +1715,7 @@ __global__ void __launch_bounds__(256) nerf_loss_kernel(int n_rays, int S, const
         s_ra += v;
         g_alpha[r] = scale * (w_alpha * 2.f * da / (float)n_rays + w_reg * dv / (float)n_rays);
     }
-    // block reduction, then ONE atomic per block and value (19 k same-address atomics serialised at L2 were 30 us of this
-    // kernel); the last block to finish turns the four sums into the loss terms the reference logs (loss.py:58-79), so no
+    // block reduction, then ONE atomic per block and value (19 k same-address atomics would serialise at L2); the last block to finish turns the four sums into the loss terms the reference logs (loss.py:58-79), so no
     // element-wise torch launches follow
     float vals[4] = {s_rgb, s_a, s_ra, s_rw};
     __shared__ float red[8][4];
@@ -1759,7 +1755,7 @@ extern "C" int ia_nerf_loss(int n_rays, int n_samples, const float* rgb, const f
     IA_REQUIRE(rgb && alpha && weights && target_rgb && target_alpha && g_rgb && g_alpha && g_weights && sums);
     cudaStream_t st = (cudaStream_t)stream;
     IA_CHECK_CUDA(cudaMemsetAsync(sums, 0, 12 * sizeof(float), st));
-    const int sms = sm_count() > 0 ? sm_count() : 148;
+    const int sms = sm_count() > 0 ? sm_count() : 132;
     nerf_loss_kernel<<<sms * 4, 256, 0, st>>>(n_rays, n_samples, rgb, alpha, weights, target_rgb, target_alpha, w_rgb, w_alpha, w_reg,
                                               scale_dev, g_rgb, g_alpha, g_weights, sums);
     IA_CHECK_CUDA(cudaPeekAtLastError());

@@ -1,4 +1,4 @@
-"""CUDA-graph capture of the two steady-state launch sequences (B200-first replacement for the reference's
+"""CUDA-graph capture of the two steady-state launch sequences (replacement for the reference's
 host-synchronous Python loops): one rendered frame and one training step.
 
 Everything inside `DNeRFModel.render_image_fast` / `training_step` is enqueued on one stream with no host

@@ -84,7 +84,7 @@ class DNeRFModel(torch.nn.Module):
     def configure_parallel(self, world_size: int):
         """Ray-sharded training over `world_size` ranks.  With 1/G of the step's rays a rank has fewer ray tiles than resident
         warps and the forward kernel's time is the critical path of its heaviest tile, so from 4 ranks on the tiles shrink to
-        one ray with 32-deep look-ahead (measured: profiles/launches_train_512*_r2.csv; results do not depend on the tile)."""
+        one ray with 32-deep look-ahead (results do not depend on the tile)."""
         self.world_size = int(world_size)
         ops.set_option("train_rays_per_warp", 1 if self.world_size >= 4 else 2)
         self.optimizer.prepare(self.world_size)
@@ -276,8 +276,8 @@ class DNeRFModel(torch.nn.Module):
 
     @torch.no_grad()
     def render_image_sharded(self, batch, img_size, rank, world, jitters, tile=2048, peer=None):
-        """One frame rendered cooperatively by `world` GPUs (BASELINE.json config 3): per-frame preparation is replicated
-        (0.1 ms), the occupancy-grid queries are sharded with one 1 MB max-all-reduce, rays are dealt round-robin in tiles
+        """One frame rendered cooperatively by `world` GPUs (BASELINE.json config 3): per-frame preparation is replicated,
+        the occupancy-grid queries are sharded with one 1 MB max-all-reduce, rays are dealt round-robin in tiles
         of `tile` rays (whole image rows) and the RGBA rows are gathered on rank 0.  `jitters` must be identical on all
         ranks.  Returns [H*W, 4] (RGBA) on every rank (on rank 0 only when the tiles do not divide evenly).
         peer (parallel.PeerFrame): both exchanges happen inside the kernels over NVLink peer memory (atomics into every
@@ -296,8 +296,7 @@ class DNeRFModel(torch.nn.Module):
         self.renderer.image_width = W if tile % (2 * W) == 0 else 0
         bg = batch["bg_color"].reshape(-1, 3)[idx] if batch.get("bg_color", None) is not None else None
         # a rank holds 1/world of the rays: keep the number of ray tiles (CTAs) of the full frame by shrinking the tile
-        # (rays per warp 4 -> 2 -> 1 at world 4 / 8; measured 0.96 -> 0.71 ms per frame at 8 GPUs,
-        # profiles/timeline_sharded_n8_r2.jsonl); results do not depend on the tile size
+        # (rays per warp 4 -> 2 -> 1 at world 4 / 8); results do not depend on the tile size
         full_rpw = ops.get_option("render_rays_per_warp")
         ops.set_option("render_rays_per_warp", getattr(self, "sharded_render_rays_per_warp", None) or sharded_rays_per_warp(full_rpw, world))
         try:

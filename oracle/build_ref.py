@@ -1,9 +1,9 @@
-"""TEST INFRASTRUCTURE: builds the REFERENCE's own CUDA extensions for sm_100 from the sources where they lie
-under /root/reference into oracle/_ref/*.so (git-ignored, shipped to the GPU box by gpurun).
+"""TEST INFRASTRUCTURE: builds the REFERENCE's own CUDA extensions for sm_90 from the sources where they lie
+under /root/reference into oracle/_ref/*.so (git-ignored; built only where the reference sources exist).
 
-They are used only by tests/ and bench.py's reference-structure leg, to pin the oracle against the reference's
-real kernels on the GPU and to time the reference's structure.  No reference source is copied into the repo:
-compilation happens in a temporary directory and only the shared objects are kept.
+They are used only by the golden-vector generators under tests/golden/ and bench.py's reference-structure leg, to
+record the reference's real kernels on the GPU and to time the reference's structure.  No reference source is copied
+into the repo: compilation happens in a temporary directory and only the shared objects are kept.
 
   fuse_cuda       deformers/fast_snarf/cuda/fuse_kernel/{fuse_cuda.cpp,fuse_cuda_kernel_fast.cu}   (unmodified)
   filter          deformers/fast_snarf/cuda/filter/{filter.cpp,filter.cu}                            (unmodified)
@@ -50,7 +50,7 @@ def build(force: bool = False) -> None:
     todo = [n for n in EXTS if force or not os.path.exists(os.path.join(OUT, f"{n}.so"))]
     if not todo:
         return
-    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "10.0")
+    os.environ.setdefault("TORCH_CUDA_ARCH_LIST", "9.0")
     os.environ["CC"] = "/usr/bin/gcc"; os.environ["CXX"] = "/usr/bin/g++"
     from torch.utils.cpp_extension import load
     for name in todo:

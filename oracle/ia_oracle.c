@@ -286,7 +286,7 @@ ORC_API void orc_filter(const float *xc, const uint8_t *valid, long M, int I, ui
 /* fp16 corner terms + fp16 running sum in the hash interpolation, fp16       */
 /* accumulator fragments (rounded per 16-wide k-block) in every MLP layer.    */
 /* It exists to BOUND how far real tcnn can be from mode 1; the deltas are   */
-/* committed in tests/golden/ngp_kat_golden.npz and profiles/parity_r2.json. */
+/* committed in tests/golden/ngp_kat_golden.npz.                             */
 /* ------------------------------------------------------------------------ */
 #define ORC_NLEVELS 16
 

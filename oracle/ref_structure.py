@@ -9,8 +9,8 @@ precompute) driven by the reference's host-side control flow, restated from
 
 with ONE substitution: tiny-cuda-nn (absent, cannot be built -- BASELINE.md §2) is replaced by this repo's
 `ia_ngp_forward` as the hash-grid + MLP evaluator.  It therefore measures "reference kernels + reference host loop +
-new network" on a B200: the closest runnable stand-in for the north_star's "reference tiny-cuda-nn path on 1xB200".
-Used by bench.py (`ref_structure` field) and tests; never by the product.
+new network" on one GPU: the closest runnable stand-in for the reference's tiny-cuda-nn path.
+Used by bench.py (`ref_structure` field) and the golden-vector generators; never by the product.
 """
 from __future__ import annotations
 

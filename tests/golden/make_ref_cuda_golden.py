@@ -1,7 +1,7 @@
-"""Runs the REFERENCE's own CUDA kernels (built from /root/reference into oracle/_ref by oracle/build_ref.py) on a
-B200 and stores small input/output vectors, so that the CPU test-suite can pin the oracle against the reference's
-real kernels.  Run on the GPU box:  gpurun -- python tests/golden/make_ref_cuda_golden.py  (writes
-gpurun_out/ref_cuda_golden.npz, then copied to tests/golden/)."""
+"""Runs the REFERENCE's own CUDA kernels (built from /root/reference into oracle/_ref by oracle/build_ref.py) on an
+H100 and stores small input/output vectors, so that the CPU test-suite can pin the oracle against the reference's
+real kernels.  Usage (needs a GPU and oracle/_ref):  python tests/golden/make_ref_cuda_golden.py OUT_DIR
+(the composite inputs are multiples of 1/256 drawn from a seeded generator, which keeps the file well under 1 MB)."""
 import os, sys
 import numpy as np, torch
 ROOT = os.path.dirname(os.path.dirname(os.path.dirname(os.path.abspath(__file__))))
@@ -32,7 +32,7 @@ fuse.fuse_broyden(xc, t(pts)[None], voxel_d, voxel_J, t(fr["tfs"])[None], torch.
                   t(subj.offset_kernel).reshape(1, 1, 3), t(subj.scale_kernel).reshape(1, 1, 3), 1e-5, 1e-1)
 mask = filt.filter(xc, valid)
 out["broyden/pts"] = pts; out["broyden/xc"] = xc[0].cpu().numpy(); out["broyden/valid"] = valid[0].cpu().numpy()
-out["broyden/mask"] = mask[0].cpu().numpy(); out["broyden/jinv"] = jinv[0].cpu().numpy()
+out["broyden/mask"] = mask[0].cpu().numpy()
 # ---- raymarch_train / raymarch_test / composite_test (raymarcher.cu) ----
 from oracle import scene as oscene
 o, dd, near, far = oscene.camera_rays(fr, 512, 512)
@@ -46,11 +46,14 @@ nears = t(near).clone(); alive = torch.arange(len(o), device="cuda")
 pts_t, dl, zz = rm.raymarch_test(t(o), t(dd), nears, t(far), alive, grid, scale, offset, step, 24)
 out["march/test_pts"] = pts_t.cpu().numpy(); out["march/test_deltas"] = dl.cpu().numpy(); out["march/test_z"] = zz.cpu().numpy()
 out["march/test_nears_after"] = nears.cpu().numpy()
-rgbv = torch.rand(pts_t.shape, device="cuda"); sig = (torch.randn(dl.shape, device="cuda") * 40)
+qr = np.random.default_rng(9)
+rgbv = t((qr.integers(0, 257, pts_t.shape) / 256).astype(np.float32))
+sig = t((np.round(qr.normal(0, 40, dl.shape) * 4) / 4).astype(np.float32))
 color = torch.zeros((len(o), 3), device="cuda"); depth = torch.zeros(len(o), device="cuda"); nohit = torch.ones(len(o), device="cuda")
 rm.composite_test(rgbv, sig, dl, zz, alive, color, depth, nohit, 0.01)
 out["comp/rgb"] = rgbv.cpu().numpy(); out["comp/sigma"] = sig.cpu().numpy(); out["comp/color"] = color.cpu().numpy()
 out["comp/depth"] = depth.cpu().numpy(); out["comp/nohit"] = nohit.cpu().numpy()
-os.makedirs(os.path.join(ROOT, "gpurun_out"), exist_ok=True)
-np.savez_compressed(os.path.join(ROOT, "gpurun_out", "ref_cuda_golden.npz"), **out)
+out_dir = sys.argv[1] if len(sys.argv) > 1 else os.path.join(ROOT, "tests", "golden")
+os.makedirs(out_dir, exist_ok=True)
+np.savez_compressed(os.path.join(out_dir, "ref_cuda_golden.npz"), **out)
 print("saved", {k: v.shape for k, v in out.items()})

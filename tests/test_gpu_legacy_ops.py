@@ -1,5 +1,5 @@
 """GPU: kernel-for-kernel raymarcher operators (ia_raymarch_train / ia_raymarch_test / ia_composite_test) against the
-outputs of the REFERENCE'S OWN kernels recorded on a B200 (tests/golden/ref_cuda_golden.npz), and the legacy
+outputs of the REFERENCE'S OWN kernels recorded on an H100 (tests/golden/ref_cuda_golden.npz), and the legacy
 `model(pts)` path of Raymarcher against the oracle's windowed host loop."""
 import os
 

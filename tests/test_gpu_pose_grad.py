@@ -154,47 +154,52 @@ def test_pose_gradients_fused_and_autograd_paths_agree():
 def test_pose_gradient_matches_finite_differences():
     """d loss / d body_pose from the implicit-differentiation kernel against central finite differences of the forward
     loss (fixed occupancy grid, fixed jitter, no noise).  Broyden's J_inv is a secant estimate, so the agreement is that
-    of the reference's own gradient definition: direction and magnitude, not digits."""
+    of the reference's own gradient definition: direction and magnitude, not digits.
+
+    One draw of 2048 rays + jitter is too small a sample for that statistic: on identical code the cosine of single draws
+    spreads from below 0.5 to 0.99 (roots that switch between initialisations make the loss piecewise smooth).  The
+    gradients are therefore summed over six independent draws (a loss over six ray batches).  The draws come from a host
+    generator: the CUDA generator's stream depends on the launch grid, i.e. on the GPU's SM count."""
     import torch
     model, batch, rgb_gt, alpha_gt, (H, W) = _gt_and_model()
     model.train()
     ys, xs = np.arange(30, 100), np.arange(40, 90)
     sel = torch.from_numpy((ys[:, None] * W + xs[None]).ravel()).cuda()
-    g = torch.Generator(device="cuda").manual_seed(7)
-    pick = sel[torch.randperm(len(sel), device="cuda", generator=g)[:2048]]
-    b = _ray_batch(batch, pick, rgb_gt, alpha_gt, 0)
     pose = batch["body_pose"].clone()
     for j, ang in ((15, 0.15), (16, -0.15), (0, 0.1), (1, -0.1), (3, 0.1)):
         pose[0, 3 * j + 2] += ang
-    jitter = torch.rand((2048, 256), device="cuda", generator=g)
     zeros = torch.zeros((2048, 256), device="cuda")
-    gj = torch.rand((64, 64, 64, 3), device="cuda", generator=g)
-
-    def loss_at(body_pose):
-        bb = dict(b); bb["body_pose"] = body_pose
-        model.deformer.prepare_deformer(bb)
-        model.net_coarse.initialize(model.deformer.bbox)
-        predicts = model.forward(bb, eval_mode=False, jitter=jitter, noise_tensor=zeros)
-        return model.loss_fn(predicts, bb)["loss"]
-
     model.deformer.fast_prepare = False   # the same (torch) SMPL path for the analytic and the differenced evaluations
-    with torch.no_grad():
-        bb = dict(b); bb["body_pose"] = pose
-        model.deformer.prepare_deformer(bb)
-        model.net_coarse.initialize(model.deformer.bbox)
-        model.global_step = 0
-        model.update_density_grid(gj)
-    theta = pose.clone().requires_grad_(True)
-    loss_at(theta).backward()
-    ga = theta.grad[0].cpu().numpy().astype(np.float64)
-    ks = np.argsort(-np.abs(ga))[:10]
     eps = 4e-3
-    fd = []
-    with torch.no_grad():
-        for k in ks:
-            e = torch.zeros_like(pose); e[0, k] = eps
-            fd.append((loss_at(pose + e).item() - loss_at(pose - e).item()) / (2 * eps))
-    fd = np.array(fd); an = ga[ks]
+    ga, fd = np.zeros(69), np.zeros(69)
+    for draw in range(6):
+        g = torch.Generator().manual_seed(draw)
+        b = _ray_batch(batch, sel[torch.randperm(len(sel), generator=g)[:2048].cuda()], rgb_gt, alpha_gt, 0)
+        jitter = torch.rand((2048, 256), generator=g).cuda()
+        gj = torch.rand((64, 64, 64, 3), generator=g).cuda()
+
+        def loss_at(body_pose):
+            bb = dict(b); bb["body_pose"] = body_pose
+            model.deformer.prepare_deformer(bb)
+            model.net_coarse.initialize(model.deformer.bbox)
+            predicts = model.forward(bb, eval_mode=False, jitter=jitter, noise_tensor=zeros)
+            return model.loss_fn(predicts, bb)["loss"]
+
+        with torch.no_grad():
+            bb = dict(b); bb["body_pose"] = pose
+            model.deformer.prepare_deformer(bb)
+            model.net_coarse.initialize(model.deformer.bbox)
+            model.global_step = 0
+            model.update_density_grid(gj)
+        theta = pose.clone().requires_grad_(True)
+        loss_at(theta).backward()
+        ga += theta.grad[0].cpu().numpy().astype(np.float64)
+        with torch.no_grad():
+            for k in range(69):
+                e = torch.zeros_like(pose); e[0, k] = eps
+                fd[k] += (loss_at(pose + e).item() - loss_at(pose - e).item()) / (2 * eps)
+    ks = np.argsort(-np.abs(ga))[:10]
+    fd = fd[ks]; an = ga[ks]
     cos = float(fd @ an / (np.linalg.norm(fd) * np.linalg.norm(an)))
     ratio = float(np.linalg.norm(an) / np.linalg.norm(fd))
     print("analytic", an, "fd", fd, "cos", cos, "ratio", ratio)

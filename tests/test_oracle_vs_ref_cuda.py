@@ -1,5 +1,5 @@
 """CPU: pins the C oracle against outputs of the REFERENCE's own CUDA kernels (fuse_broyden, filter, precompute,
-raymarch_train/test, composite_test) recorded on a B200 by tests/golden/make_ref_cuda_golden.py."""
+raymarch_train/test, composite_test) recorded on an H100 by tests/golden/make_ref_cuda_golden.py."""
 import os
 
 import numpy as np

@@ -1,6 +1,6 @@
-"""CPU: the reference's module paths resolve to the B200 mirror classes (SURVEY.md §8b).
+"""CPU: the reference's module paths resolve to the instantavatar_b200 mirror classes (SURVEY.md §8b).
 
-Every `_target_` string of /root/reference/confs/{renderer,deformer,network}/*.yaml and of the `model` / `loss` nodes of
+Every `_target_` string of the reference's confs/{renderer,deformer,network}/*.yaml and of the `model` / `loss` nodes of
 confs/SNARF_NGP*.yaml is resolved with importlib (no Hydra) through the `instant_avatar` alias package, the classes are
 checked to be the instantavatar_b200 ones, and the classes that construct without a GPU are instantiated from the
 reference's own YAML argument sets."""
@@ -44,23 +44,19 @@ def test_target_resolves_to_the_mirror(conf, target, kwargs):
     assert cls is _resolve(MIRROR[target]), (target, cls)
 
 
-def test_targets_are_the_reference_files_targets():
-    """the committed list above equals what the reference's YAML files hold (only where /root/reference is mounted)"""
-    ref = "/root/reference"
-    if not os.path.isdir(ref):
-        pytest.skip("reference tree not mounted (GPU box)")
-    import re
-    found = set()
-    for sub in ("renderer", "deformer", "network"):
-        d = os.path.join(ref, "confs", sub)
-        for f in sorted(os.listdir(d)):
-            for m in re.finditer(r"_target_:\s*(\S+)", open(os.path.join(d, f)).read()):
-                found.add((f"confs/{sub}/{f}", m.group(1)))
+def test_targets_are_the_reference_files_targets(golden_dir):
+    """the committed list above equals what the reference's YAML files hold (recorded in
+    tests/golden/reference_conf_targets.json by tests/golden/make_reference_conf_targets.py)"""
+    import json
+    rec = json.load(open(os.path.join(golden_dir, "reference_conf_targets.json")))
+    found = {(c, t) for c, t in rec["by_subdir"]}
     committed = {(c, t) for c, t, _ in TARGETS if c.split("/")[1] in ("renderer", "deformer", "network")}
     assert found == committed, found ^ committed
-    for f in ("SNARF_NGP.yaml", "SNARF_NGP_refine.yaml", "SNARF_NGP_fitting.yaml", "demo.yaml"):
-        for m in re.finditer(r"_target_:\s*(\S+)", open(os.path.join(ref, "confs", f)).read()):
-            assert m.group(1) in MIRROR, (f, m.group(1))
+    assert set(rec["top_level"]) == {f"confs/{f}" for f in ("SNARF_NGP.yaml", "SNARF_NGP_refine.yaml", "SNARF_NGP_fitting.yaml", "demo.yaml")}
+    for f, ts in rec["top_level"].items():
+        assert ts, f
+        for t in ts:
+            assert t in MIRROR, (f, t)
 
 
 def test_instantiate_cpu_constructible_targets():
@@ -96,22 +92,26 @@ def test_reference_import_statements():
     assert DensityGrid.__module__.startswith("instantavatar_b200") and SMPLParamEmbedding.__module__.startswith("instantavatar_b200")
 
 
-def test_reference_ngp_file_runs_on_the_tinycudann_shim():
-    """the reference's OWN models/networks/ngp.py, loaded from /root/reference by path, builds on the in-repo `tinycudann`
-    module: same sub-module names and flat parameter sizes (CPU: construction only; the forward is a GPU test)"""
-    import importlib.util
-    import sys
-    ref = "/root/reference/instant_avatar/models/networks/ngp.py"
-    if not os.path.exists(ref):
-        pytest.skip("reference tree not mounted (GPU box)")
-    import tinycudann  # the shim must win the import inside the reference file
+def test_reference_ngp_file_runs_on_the_tinycudann_shim(golden_dir):
+    """the tiny-cuda-nn modules the reference's models/networks/ngp.py constructs (NeRFNGPNet.__init__: attribute, class and
+    keyword arguments, recorded in tests/golden/reference_ngp_modules.json by tests/golden/make_reference_ngp_modules.py)
+    build on the in-repo `tinycudann` module: same sub-module names and flat parameter sizes as tcnn, and the same as the
+    mirror class (CPU: construction only; the forward is a GPU test)"""
+    import json
+    import torch
+    import tinycudann  # the shim must win the import the reference file makes
     assert "ia_b200" in tinycudann.__version__
-    spec = importlib.util.spec_from_file_location("_ref_ngp_under_shim", ref)
-    mod = importlib.util.module_from_spec(spec)
-    spec.loader.exec_module(mod)
-    from instantavatar_b200.config import Cfg
-    net = mod.NeRFNGPNet(Cfg({"center": [0, -0.3, 0], "scale": [2.5, 2.5, 2.5]}))
+    rec = json.load(open(os.path.join(golden_dir, "reference_ngp_modules.json")))
+    assert rec["class"] == "NeRFNGPNet" and [m["attr"] for m in rec["modules"]] == ["encoder", "color_net"]
+    net = torch.nn.Module()
+    for m in rec["modules"]:
+        setattr(net, m["attr"], getattr(tinycudann, m["class"])(**m["kwargs"]))
+    for b in rec["buffers"]:
+        net.register_buffer(b, torch.zeros(3))
     sizes = {k: v.numel() for k, v in net.named_parameters()}
     assert sizes == {"encoder.params": 3072 + 2 * 6513496, "color_net.params": 6144}
     assert set(dict(net.named_buffers())) == {"center", "scale"}
-    sys.modules.pop("_ref_ngp_under_shim", None)
+    from instantavatar_b200.config import instantiate
+    mirror = instantiate({"_target_": "instant_avatar.models.networks.ngp.NeRFNGPNet",
+                          "opt": {"use_viewdir": False, "cond_dim": 0, "center": [0, -0.3, 0], "scale": [2.5, 2.5, 2.5]}})
+    assert {k: v.numel() for k, v in mirror.named_parameters()} == sizes

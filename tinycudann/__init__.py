@@ -11,7 +11,7 @@ The reference's network file imports `tinycudann as tcnn` and builds exactly two
 This module provides those two classes with tiny-cuda-nn's Python surface for that use: `nn.Module`s with ONE flat fp32
 `params` Parameter (tcnn ordering: [MLP weights | grid] / [W3 | W4 | W5], row-major [out, in] matrices), `forward(x)` on
 float inputs returning fp16, differentiable in `params` and in the input, gradients computed with an internal loss scale
-of 128 (tcnn's default).  With it on the path, the reference's ngp.py runs unmodified on the B200 kernels
+of 128 (tcnn's default).  With it on the path, the reference's ngp.py runs unmodified on the H100 kernels
 (ia_tcnn_encoder_* / ia_tcnn_mlp_*).  Any other configuration raises NotImplementedError: only what the hot path uses is
 built.  There is no CPU fallback."""
 from __future__ import annotations
