@@ -366,10 +366,16 @@ struct CompBwdArgs {
 // original order with operands broadcast by shuffle, each lane keeping the values of its own slot.  (Thread per ray, a
 // 256-slot ray would be 2 x 32 dependent load round trips.)  Same list layout as before:
 // a ray's samples occupy one contiguous block in slot order.
+// The reverse sweep reads each slot's transmittance as the forward sweep computed it (kept in shared memory), never by
+// dividing back from the final one: once sum(relu(sigma) * dt) exceeds ~87 that final fp32 T is denormal or zero, and
+// division would lose every gradient of the ray, front surface included.  It also makes w = alpha * T bit-identical to
+// the forward's weights.
 __global__ void __launch_bounds__(256) composite_bwd_kernel(CompBwdArgs a) {
+    __shared__ float s_tb[8][IA_MAX_SAMPLES];  // per warp (8 per 256-thread block): T before each slot
     const int lane = threadIdx.x & 31;
     const int ray = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
     if (ray >= a.n_rays) return;
+    float* __restrict__ tb = s_tb[threadIdx.x >> 5];  // each lane writes and reads only its own slots: no barrier
     const int cnt = a.s_count[ray];
     if (cnt == 0) return;
     const float dt = (a.far[ray] - a.near[ray]) / (float)IA_MAX_SAMPLES;
@@ -387,7 +393,7 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(CompBwdArgs a) {
     if (a.g_alpha) ga = a.g_alpha[ray];
     float b[3] = {1.f, 1.f, 1.f};
     if (a.bg) { b[0] = a.bg[ray * 3]; b[1] = a.bg[ray * 3 + 1]; b[2] = a.bg[ray * 3 + 2]; }
-    // ---- forward sweep: T after the last sample, number of samples that reached the network ----
+    // ---- forward sweep: T before every sample (the forward's recurrence), number of samples that reached the network ----
     float T = 1.f;
     int nvalid = 0;
     for (int s0 = 0; s0 < cnt; s0 += 32) {
@@ -400,14 +406,18 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(CompBwdArgs a) {
         const float f = (1.0f - al) + 1e-10f;
         nvalid += __popc(__ballot_sync(kFull, in && bs >= 0));
         const int m = min(32, cnt - s0);
-        for (int j = 0; j < m; j++) T = T * __shfl_sync(kFull, f, j);
+        float my_T = 0.f;
+        for (int j = 0; j < m; j++) {
+            if (j == lane) my_T = T;
+            T = T * __shfl_sync(kFull, f, j);
+        }
+        if (in) tb[s] = my_T;
     }
     if (nvalid == 0) return;
     int start = 0;
     if (lane == 0) start = atomicAdd(a.l_count, nvalid);
     start = __shfl_sync(kFull, start, 0);
     float S = gc[0] * b[0] + gc[1] * b[1] + gc[2] * b[2];  // dL/dT entering the next sample; starts at the background term
-    float Tn = T;                                          // T after sample s
     int above = 0;                                         // valid samples in the groups already processed (higher slots)
     for (int s0 = ((cnt - 1) / 32) * 32; s0 >= 0; s0 -= 32) {
         const int s = s0 + lane;
@@ -426,16 +436,13 @@ __global__ void __launch_bounds__(256) composite_bwd_kernel(CompBwdArgs a) {
         const float f = (1.0f - al) + 1e-10f;
         const float Gs = gc[0] * c0 + gc[1] * c1 + gc[2] * c2 + gd * zz + ga + gw;
         const int m = min(32, cnt - s0);
-        float my_Tb = 0.f, my_dLdal = 0.f;
+        const float my_Tb = in ? tb[s] : 0.f;  // T before this lane's sample
+        float my_S = 0.f;                      // dL/dT after this lane's sample
         for (int j = m - 1; j >= 0; j--) {
-            const float fj = __shfl_sync(kFull, f, j), Gj = __shfl_sync(kFull, Gs, j), aj = __shfl_sync(kFull, al, j);
-            const float Tb = Tn / fj;  // T before sample j
-            const float dLdf = S * Tb;
-            const float dLdal = Gj * Tb - dLdf;
-            S = S * fj + Gj * aj;
-            Tn = Tb;
-            if (j == lane) { my_Tb = Tb; my_dLdal = dLdal; }
+            if (j == lane) my_S = S;
+            S = S * __shfl_sync(kFull, f, j) + __shfl_sync(kFull, Gs, j) * __shfl_sync(kFull, al, j);
         }
+        const float my_dLdal = Gs * my_Tb - my_S * my_Tb;
         const bool valid = in && bs >= 0;
         const unsigned vm = __ballot_sync(kFull, valid);
         if (valid) {
