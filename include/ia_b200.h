@@ -32,6 +32,18 @@ extern "C" {
 
 typedef void* ia_stream_t; /* cudaStream_t */
 
+/* Per-frame state of the nearest-vertex deformer (deformers/smpl_deformer.py:87-137, `deformer=smpl`): a sample x in the
+ * root frame takes its nearest posed vertex v (squared fp32 distance dx*dx + dy*dy + dz*dz, ties to the lower index) and is
+ * valid iff d2 < (float)(threshold * threshold); its canonical point is table[v] . [x, 1].  `grid` is a caller-owned
+ * workspace of ia_nv_workspace_bytes(n_verts) bytes filled by ia_nv_grid_build from `verts`. */
+typedef struct IaNearestVertex {
+    void* grid;              /* vertex bucket grid (ia_nv_grid_build) */
+    const float* verts;      /* [n_verts][3] posed vertices, root frame */
+    const float* table;      /* [n_verts][12] rows 0..2 of T_inv[v] (3x4, row-major) */
+    int32_t n_verts;
+    double threshold;        /* smpl_deformer.py `threshold` (0.05) */
+} IaNearestVertex;
+
 /* Per-frame read-only state of the fused kernels. */
 typedef struct IaScene {
     const float* field;      /* [D][H][W][24] fp32: blended 3x4 LBS transform of voxel x followed by that of voxel x+1 (zeros at x = W-1); 96-B records written by ia_precompute */
@@ -46,6 +58,11 @@ typedef struct IaScene {
     const void* mlp_h;       /* half[IA_MLP_HALFS] padded MLP weights (ia_params_to_half) */
     const float* net_center; /* [3] NeRFNGPNet.center (ngp.py:64-71) */
     const float* net_scale;  /* [3] NeRFNGPNet.scale */
+    /* [host] nullable.  Set: the deform stage is the nearest-vertex search instead of Fast-SNARF's root finding, and
+     * field / offset_k / scale_k / tfs / D / H / W are not read.  Supported by ia_render_fwd, ia_occupancy_query(_ordered),
+     * ia_deform_query and ia_train_fwd_split; ia_train_fwd, ia_render_fwd_peer, ia_occupancy_query_peer, ia_broyden and
+     * ia_pose_grad return IA_EINVAL (the pose gradient is ia_nv_pose_grad). */
+    const IaNearestVertex* nv;
 } IaScene;
 
 /* Work counters accumulated by the kernels (device memory, caller zeroes). */
@@ -97,6 +114,17 @@ int ia_voxelize_weights(const float* verts, const float* vert_weights, int n_ver
  * (deformers/smpl_deformer.py:94-95; third_parties/pytorch3d/ops.py:123-206 contract: squared distance, ties keep the
  * earlier vertex).  pts [n][3], verts [n_verts][3] -> idx_out [n] int32, dist2_out [n]. */
 int ia_knn1(const float* pts, int n, const float* verts, int n_verts, int* idx_out, float* dist2_out, ia_stream_t stream);
+
+/* Nearest-vertex deformer, per frame: one CTA buckets nv->verts into a uniform grid in nv->grid (bounds, per-cell counts,
+ * scan, scatter; cell edge >= 1.01 * threshold, widened if the cell count would exceed the workspace's capacity; the grid
+ * is padded by one cell on every side).  No host synchronisation.  Every vertex within `threshold` of a point lies in the
+ * 3x3x3 cells around it, so the search is exact for every valid point, and points outside the grid are invalid. */
+size_t ia_nv_workspace_bytes(int n_verts);
+int ia_nv_grid_build(const IaNearestVertex* nv /*[host]*/, ia_stream_t stream);
+/* The grid search on its own (the grid analogue of ia_knn1): pts [n][3] -> idx_out [n] int32 and dist2_out [n] of the
+ * nearest vertex for valid points (d2 < threshold^2; same index and bit-identical d2 as ia_knn1), -1 and +inf otherwise. */
+int ia_nv_nearest(const IaNearestVertex* nv /*[host]*/, const float* pts, int n, int* idx_out, float* dist2_out,
+                  ia_stream_t stream);
 
 /* Per-frame bone transforms in one launch.  Replaces, for everything the renderer consumes, the SMPL forward + tfs
  * algebra of SNARFDeformer.prepare_deformer (deformers/snarf_deformer.py:79-86; smplx/lbs.py:295-329 Rodrigues,
@@ -313,6 +341,17 @@ int ia_ngp_input_grad(const IaScene* scene /*[host]*/, const float* x, const flo
  * lbs_voxel [24][D][H][W] (ForwardDeformer.lbs_voxel_final). */
 int ia_pose_grad(const IaScene* scene /*[host]*/, const float* lbs_voxel, const float* xd, const int8_t* best,
                  const float* denc, const int* count, int capacity, float* grad_tfs, ia_stream_t stream);
+
+/* Pose gradient of the nearest-vertex deformer (scene->nv set).  For each of the first min(*count, capacity) list samples
+ * of ia_composite_bwd with best >= 0: l_rz [capacity][3] holds (ray index, z, 0) -- what ia_composite_bwd writes into l_xd
+ * when it is given the rays rays_o[i] = (i, 0, 0), rays_d[i] = (0, 1, 0) (z * 0 + i and z * 1 + 0 are exact).  The posed
+ * point x = z * rays_d[ray] + rays_o[ray] is recomputed as the forward generated it, the forward's nearest-vertex search is
+ * re-run from it (bit-identical), g = d loss / d x_c is formed from denc (ia_ngp_backward) as ia_ngp_input_grad does, and
+ * accumulated (+=): grad_table [n_verts][3][4] += g (x) [x, 1] (d loss / d nv->table); grad_rays_o [n_rays][3] += T^T g and
+ * grad_rays_d [n_rays][3] += z T^T g with T = table[v][:3][:3] (both nullable: d loss / d rays through x = z d + o). */
+int ia_nv_pose_grad(const IaScene* scene /*[host]*/, const float* rays_o, const float* rays_d, int n_rays, const float* l_rz,
+                    const int8_t* best, const float* denc, const int* count, int capacity, float* grad_table,
+                    float* grad_rays_o /*nullable*/, float* grad_rays_d /*nullable*/, ia_stream_t stream);
 
 /* NeRFLoss forward + analytic backward in one pass (instant_avatar/utils/loss.py:53-79):
  * loss = w_rgb mse(rgb) + w_alpha mse(alpha) + w_reg (mean reg(alpha) + mean reg(weights) + 2*0.313262),

@@ -27,7 +27,13 @@ SYMBOLS = [
     "ia_mlp_to_half", "ia_raymarch_train", "ia_raymarch_test", "ia_composite_test", "ia_smpl_tfs", "ia_nerf_loss", "ia_pose_grad", "ia_knn1", "ia_smpl_tfs_backward", "ia_ngp_input_grad", "ia_voxelize_weights", "ia_render_fwd", "ia_deform_query", "ia_broyden", "ia_ngp_forward", "ia_transform_rays", "ia_mlp_to_half_from_half", "ia_grad_poison_shards", "ia_gather_ceiling", "ia_tcnn_backward_scratch_bytes", "ia_tcnn_encoder_forward",
     "ia_tcnn_encoder_backward", "ia_tcnn_mlp_forward", "ia_tcnn_mlp_backward", "ia_render_fwd_peer", "ia_occupancy_query_peer", "ia_peer_reduce_check",
     "ia_peer_flags_to_found", "ia_adam_step_dev_peer", "ia_occupancy_query_ordered", "ia_train_fwd_split", "ia_train_fwd_workspace_bytes",
+    "ia_nv_workspace_bytes", "ia_nv_grid_build", "ia_nv_nearest", "ia_nv_pose_grad",
 ]
+
+
+class IaNearestVertex(C.Structure):
+    _fields_ = [("grid", C.c_void_p), ("verts", C.c_void_p), ("table", C.c_void_p), ("n_verts", C.c_int32),
+                ("threshold", C.c_double)]
 
 
 class IaScene(C.Structure):
@@ -36,6 +42,7 @@ class IaScene(C.Structure):
         ("offset_k", C.c_void_p), ("scale_k", C.c_void_p), ("tfs", C.c_void_p),
         ("occ_bits", C.c_void_p), ("G", C.c_int32), ("occ_aabb", C.c_void_p),
         ("table_h", C.c_void_p), ("mlp_h", C.c_void_p), ("net_center", C.c_void_p), ("net_scale", C.c_void_p),
+        ("nv", C.POINTER(IaNearestVertex)),
     ]
 
 
@@ -66,6 +73,7 @@ def lib():
         _lib.ia_render_workspace_bytes.restype = C.c_size_t
         _lib.ia_tcnn_backward_scratch_bytes.restype = C.c_size_t
         _lib.ia_train_fwd_workspace_bytes.restype = C.c_size_t
+        _lib.ia_nv_workspace_bytes.restype = C.c_size_t
         for s in SYMBOLS:
             getattr(_lib, s)  # fail loudly on a stale library
         if _lib.ia_abi_version() != 1:

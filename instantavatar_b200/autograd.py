@@ -5,7 +5,10 @@ The reference differentiates ~20 ATen ops + two tiny-cuda-nn modules (SURVEY.md 
 loss consumes (rgb, depth, alpha and the dense per-sample weights) and produces gradients for the two flat parameter
 tensors `encoder.params` / `color_net.params`.  When the bone transforms `tfs` carry an autograd history (pose
 optimisation, DNeRF.py:112-127 with `optimize_SMPL.enable`), `ia_pose_grad` additionally returns d loss / d tfs -- the
-implicit-differentiation gradient of deformers/fast_snarf/deformer_torch.py:50-67.
+implicit-differentiation gradient of deformers/fast_snarf/deformer_torch.py:50-67 (the rays are constants there: the
+SNARF w2s is detached).  With the nearest-vertex deformer (SMPLDeformer) the pose leaf is its [V,12] table of T_inv rows,
+and the root-frame rays carry the global rotation and translation (smpl_deformer.py:78-85 rotates and shifts them by
+w2s); `ia_nv_pose_grad` returns d loss / d table and, when the rays have an autograd history, d loss / d rays_o, rays_d.
 """
 from __future__ import annotations
 
@@ -23,6 +26,10 @@ class _RenderTrain(torch.autograd.Function):
         out, saved = ops.train_fwd(scene, rays_o, rays_d, near, far, bg, jitter, noise, stats)
         ctx.scene, ctx.saved, ctx.misc = scene, saved, (near, far, bg, noise)
         ctx.pose = (rays_o, rays_d, lbs_voxel, tfs.shape) if tfs is not None and tfs.requires_grad else None
+        ctx.nv = scene.nv is not None
+        ctx.ray_grad = ctx.nv and (ctx.needs_input_grad[3] or ctx.needs_input_grad[4])
+        if ctx.nv and ctx.pose is None and ctx.ray_grad:
+            ctx.pose = (rays_o, rays_d, None, None)
         ctx.frozen = not (enc_params.requires_grad or col_params.requires_grad)  # pose refinement with a fixed network
         ctx.shapes = (enc_params.shape, col_params.shape)
         ctx.accum = accum  # optional persistent (grad_enc, grad_col) buffers to accumulate into
@@ -33,8 +40,11 @@ class _RenderTrain(torch.autograd.Function):
         near, far, bg, noise = ctx.misc
         dev = near.device
         pose = ctx.pose
-        lists = ops.composite_bwd(near, far, bg, noise, ctx.saved, g_rgb, g_depth, g_alpha, g_weights,
-                                  rays=pose[:2] if pose is not None else None)
+        if pose is not None and ctx.nv:   # list samples as (ray index, z): ia_nv_pose_grad recomputes the posed points
+            list_rays = ops.ray_slot_codes(near.numel(), dev)
+        else:
+            list_rays = pose[:2] if pose is not None else None
+        lists = ops.composite_bwd(near, far, bg, noise, ctx.saved, g_rgb, g_depth, g_alpha, g_weights, rays=list_rays)
         l_xc, l_ds, l_dc, l_count = lists[:4]
         denc = torch.empty((l_xc.shape[0], 32), device=dev, dtype=torch.float32) if pose is not None else None
         if ctx.frozen:
@@ -47,14 +57,24 @@ class _RenderTrain(torch.autograd.Function):
             g_enc = torch.zeros(ctx.shapes[0], device=dev, dtype=torch.float32)
             g_col = torch.zeros(ctx.shapes[1], device=dev, dtype=torch.float32)
         ops.ngp_backward(ctx.scene, l_xc, l_ds, l_dc, l_count, g_enc, g_col, GRAD_SCALE, denc)
-        g_tfs = None
-        if pose is not None:
+        g_tfs = g_o = g_d = None
+        if pose is not None and ctx.nv:
+            rays_o, rays_d = pose[:2]
+            table = ctx.scene.nv.table
+            g_tfs = torch.zeros(table.shape, device=dev, dtype=torch.float32)
+            if ctx.ray_grad:
+                g_o = torch.zeros(rays_o.shape, device=dev, dtype=torch.float32)
+                g_d = torch.zeros(rays_d.shape, device=dev, dtype=torch.float32)
+            ops.nv_pose_grad(ctx.scene, rays_o.detach(), rays_d.detach(), lists[4], lists[5], denc, l_count, g_tfs, g_o, g_d)
+            if pose[3] is None:
+                g_tfs = None
+        elif pose is not None:
             g_tfs = torch.zeros((24, 4, 4), device=dev, dtype=torch.float32)
             ops.pose_grad(ctx.scene, pose[2], lists[4], lists[5], denc, l_count, g_tfs)
             g_tfs = g_tfs.reshape(pose[3])
         if ctx.accum is not None or ctx.frozen:
-            return (None,) * 12 + (g_tfs, None)
-        return (g_enc, g_col) + (None,) * 10 + (g_tfs, None)
+            return (None,) * 3 + (g_o, g_d) + (None,) * 7 + (g_tfs, None)
+        return (g_enc, g_col, None, g_o, g_d) + (None,) * 7 + (g_tfs, None)
 
 
 def render_train_fused(renderer, deformer, net, rays, noise, bg_color, jitter=None, noise_tensor=None, stats=None):
@@ -64,17 +84,23 @@ def render_train_fused(renderer, deformer, net, rays, noise, bg_color, jitter=No
     scene = deformer.scene(net, grid.occupancy_bits(), grid.aabb6())
     rays_o = rays.o.reshape(-1, 3).float().contiguous()
     rays_d = rays.d.reshape(-1, 3).float().contiguous()
-    near = rays.near.reshape(-1).float().contiguous()
-    far = rays.far.reshape(-1).float().contiguous()
+    near = rays.near.reshape(-1).float().contiguous().detach()   # the interval length far - near = 2 carries no gradient
+    far = rays.far.reshape(-1).float().contiguous().detach()
+    if scene.nv is None:   # SNARF: the rays are constants of the fused path
+        rays_o, rays_d = rays_o.detach(), rays_d.detach()
     n = near.numel()
     if jitter is None:
         jitter = torch.rand((n, 256), device=near.device)
     if noise_tensor is None and noise > 0:
         noise_tensor = noise * torch.randn((n, 256), device=near.device)
     bg = bg_color.reshape(-1, 3).float().contiguous() if bg_color is not None else None
+    if scene.nv is not None:   # nearest-vertex deformer: the pose leaf is the T_inv table
+        pose_leaf, lbs_voxel = deformer.nv_table, None
+    else:
+        pose_leaf, lbs_voxel = deformer.tfs, deformer.deformer.lbs_voxel_final
     rgb, depth, alpha, weights = _RenderTrain.apply(net.encoder.params, net.color_net.params, scene, rays_o, rays_d, near, far, bg,
                                                     jitter.contiguous(), noise_tensor.contiguous() if noise_tensor is not None else None, stats,
-                                                    net.grad_buffers(), deformer.tfs, deformer.deformer.lbs_voxel_final)
+                                                    net.grad_buffers(), pose_leaf, lbs_voxel)
     return {
         "rgb_coarse": rgb.reshape(rays.o.shape),
         "depth_coarse": depth.reshape(rays.near.shape),

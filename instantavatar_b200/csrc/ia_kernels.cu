@@ -4,6 +4,8 @@
 #include <stdio.h>
 #include <string.h>
 
+#include <type_traits>
+
 #include "ia_warp_eval.cuh"
 
 using namespace ia;
@@ -53,13 +55,14 @@ struct RenderWarpExtra {
     int bo[32];
 };
 
-template <int kWarps>
+// kNV: nearest-vertex deform stage (warp_eval_nv), one candidate per sample
+template <int kWarps, bool kNV = false>
 struct RenderSmem {
     __align__(128) uint32_t occ[64 * 64 * 64 / 32];
     __align__(16) __half W[kMlpHalfs];
     FrameConst fc;
     __align__(8) uint64_t mbar;
-    WarpScratch<false> ws[kWarps];
+    std::conditional_t<kNV, WarpScratchNV, WarpScratch<false>> ws[kWarps];
     RenderWarpExtra wx[kWarps];
 };
 
@@ -102,10 +105,10 @@ __device__ __forceinline__ int tile_ray(int tile, int rl, bool tiled, int image_
 // Planning pass (longest-processing-time-first scheduling of the fused kernel): counts the occupied steps of every
 // ray (the scan of raymarcher.cu:13-73 without evaluating anything), reduces them per tile, and writes the
 // background result of tiles that cannot produce a sample.  The per-tile cost feeds order_tiles_kernel.
-template <int kRays>
+template <int kRays, bool kNV = false>
 __global__ void __launch_bounds__(256) render_plan_kernel(const __grid_constant__ RenderArgs a, int* __restrict__ cost) {
     __shared__ FrameConst fc;
-    load_frame_const(fc, a.sd);
+    load_frame_const<kNV>(fc, a.sd);
     __syncthreads();
     constexpr int kTileW = kRays == 32 ? 8 : (kRays >= 8 ? 4 : (kRays >= 2 ? 2 : 1));
     constexpr int kTileH = kRays / kTileW;
@@ -203,13 +206,13 @@ __global__ void __launch_bounds__(1024) order_tiles_kernel(const int* __restrict
 // kRays rays per warp, each marched kDepth = 32/kRays steps ahead (lane = depth * kRays + ray): the batch of 32
 // samples a warp evaluates stays spatially coherent (neighbouring pixels x consecutive steps) while the number of
 // independent work units grows by kDepth -- there are fewer hit rays in a 512^2 frame than resident lanes.
-template <int kWarps, int kRays>
+template <int kWarps, int kRays, bool kNV = false>
 __global__ void __launch_bounds__(kWarps * 32, 1) render_fwd_kernel(const __grid_constant__ RenderArgs a) {
     constexpr int kDepth = 32 / kRays;
     constexpr int kTileW = kRays == 32 ? 8 : (kRays >= 8 ? 4 : (kRays >= 2 ? 2 : 1));
     constexpr int kTileH = kRays / kTileW;
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    RenderSmem<kWarps>& sm = *reinterpret_cast<RenderSmem<kWarps>*>(smem_raw);
+    RenderSmem<kWarps, kNV>& sm = *reinterpret_cast<RenderSmem<kWarps, kNV>*>(smem_raw);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int G = a.sd.s.G;
     // ---- prologue: TMA-engine bulk copies of the occupancy bitfield and the MLP weights -------------
@@ -220,7 +223,7 @@ __global__ void __launch_bounds__(kWarps * 32, 1) render_fwd_kernel(const __grid
         bulk_g2s(sm.occ, a.sd.s.occ_bits, occ_bytes, &sm.mbar);
         bulk_g2s(sm.W, a.sd.s.mlp_h, kMlpHalfs * 2, &sm.mbar);
     }
-    load_frame_const(sm.fc, a.sd);
+    load_frame_const<kNV>(sm.fc, a.sd);
     __syncthreads();
     mbar_wait(&sm.mbar, 0);
 
@@ -232,7 +235,7 @@ __global__ void __launch_bounds__(kWarps * 32, 1) render_fwd_kernel(const __grid
    
     ctx.fc = &sm.fc;
     ctx.hl = &a.sd.hl;
-    WarpScratch<false>& ws = sm.ws[warp];
+    auto& ws = sm.ws[warp];
     RenderWarpExtra& wx = sm.wx[warp];
     const FrameConst& fc = sm.fc;
     const int* cbox = reinterpret_cast<const int*>(a.sd.s.occ_bits + G * G * G / 32);  // occupied-cell box
@@ -319,7 +322,11 @@ __global__ void __launch_bounds__(kWarps * 32, 1) render_fwd_kernel(const __grid
             if (!__any_sync(kFull, sact)) continue;
             st_samples += sact ? 1u : 0u;
             SampleOut so;
-            warp_eval_samples<false>(ctx, ws, sact, sx, sy, sz, true, lane, so, st_gather, st_roots, st_load, st_hash);
+            if constexpr (kNV) {
+                warp_eval_nv(ctx, a.sd.nv, ws, sact, sx, sy, sz, true, lane, so, st_roots, st_hash);
+            } else {
+                warp_eval_samples<false>(ctx, ws, sact, sx, sy, sz, true, lane, so, st_gather, st_roots, st_load, st_hash);
+            }
             // ---- composite in sample order (raymarcher.cu:200-235) ----
             ws.res[lane][0] = so.sigma; ws.res[lane][1] = so.r; ws.res[lane][2] = so.g; ws.res[lane][3] = so.b;
             wx.bt[lane] = stt; wx.bo[lane] = sact ? sown : -1;
@@ -401,29 +408,30 @@ struct QueryArgs {
     int lanes_per_sample;  // point mode: 1 / 2 / 4 lanes share a point's 13 root finds (narrow batches); 0 = pick from the load
 };
 
-template <int kWarps, bool kKeepXc>
+template <int kWarps, bool kKeepXc, bool kNV = false>
 struct QuerySmem {
     __align__(16) __half W[kMlpHalfs];
     FrameConst fc;
     __align__(8) uint64_t mbar;
-    WarpScratch<kKeepXc> ws[kWarps];
+    std::conditional_t<kNV, WarpScratchNV, WarpScratch<kKeepXc>> ws[kWarps];
 };
 
 // kKeepXc: the canonical point of the winning candidate is an output (xc_best; training-time queries); the occupancy
 // passes do not need it, which frees 5 KB of shared memory per warp => more resident warps per SM
 // kDynLanes: lanes per point chosen at run time (a.lanes_per_sample); the default occupancy-pass instantiation keeps the
 // one-lane-per-point code with a literal 1
-template <int kWarps, bool kKeepXc, bool kDynLanes = kKeepXc>
+// kNV: nearest-vertex deform stage (warp_eval_nv, one lane per point)
+template <int kWarps, bool kKeepXc, bool kDynLanes = kKeepXc, bool kNV = false>
 __global__ void __launch_bounds__(kWarps * 32, 1) deform_query_kernel(const __grid_constant__ QueryArgs a) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    QuerySmem<kWarps, kKeepXc>& sm = *reinterpret_cast<QuerySmem<kWarps, kKeepXc>*>(smem_raw);
+    QuerySmem<kWarps, kKeepXc, kNV>& sm = *reinterpret_cast<QuerySmem<kWarps, kKeepXc, kNV>*>(smem_raw);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     if (threadIdx.x == 0) {
         mbar_init(&sm.mbar, 1);
         mbar_expect_tx(&sm.mbar, kMlpHalfs * 2);
         bulk_g2s(sm.W, a.sd.s.mlp_h, kMlpHalfs * 2, &sm.mbar);
     }
-    load_frame_const(sm.fc, a.sd);
+    load_frame_const<kNV>(sm.fc, a.sd);
     __syncthreads();
     mbar_wait(&sm.mbar, 0);
     EvalCtx ctx;
@@ -491,7 +499,9 @@ __global__ void __launch_bounds__(kWarps * 32, 1) deform_query_kernel(const __gr
             }
         }
         SampleOut so;
-        if constexpr (kDynLanes) {
+        if constexpr (kNV) {
+            warp_eval_nv(ctx, a.sd.nv, sm.ws[warp], act, x, y, z, a.eval_mode != 0, lane, so, st_roots, st_hash);
+        } else if constexpr (kDynLanes) {
             warp_eval_samples<kKeepXc>(ctx, sm.ws[warp], act, x, y, z, a.eval_mode != 0, lane, so, st_gather, st_roots, st_load, st_hash, k);
         } else {
             warp_eval_samples<kKeepXc>(ctx, sm.ws[warp], act, x, y, z, a.eval_mode != 0, lane, so, st_gather, st_roots, st_load, st_hash);
@@ -969,12 +979,12 @@ size_t ia_render_workspace_bytes(int n_rays) { return 256 + 2 * sizeof(int) * (s
 
 }  // extern "C"
 
-template <int kWarps, int kRays>
+template <int kWarps, int kRays, bool kNV = false>
 static int launch_render(RenderArgs& a, bool plan, int* ws_cost, int* ws_order, cudaStream_t st) {
-    const size_t smem = sizeof(RenderSmem<kWarps>);
+    const size_t smem = sizeof(RenderSmem<kWarps, kNV>);
     static PerDeviceFlag attr_set;
     if (!attr_set.get()) {
-        IA_CHECK_CUDA(cudaFuncSetAttribute(render_fwd_kernel<kWarps, kRays>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        IA_CHECK_CUDA(cudaFuncSetAttribute(render_fwd_kernel<kWarps, kRays, kNV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set.set();
     }
     const int n_tiles = (a.n_rays + kRays - 1) / kRays;
@@ -983,33 +993,38 @@ static int launch_render(RenderArgs& a, bool plan, int* ws_cost, int* ws_order, 
     grid = min(grid, (n_tiles + kWarps - 1) / kWarps);
     if (plan) {
         const long threads = (long)n_tiles * kRays;
-        render_plan_kernel<kRays><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(a, ws_cost);
+        render_plan_kernel<kRays, kNV><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(a, ws_cost);
         order_tiles_kernel<<<1, 1024, 0, st>>>(ws_cost, n_tiles, ws_order, a.tile_counter + 1);
         a.tile_order = ws_order;
         a.n_active = a.tile_counter + 1;
     }
-    render_fwd_kernel<kWarps, kRays><<<grid, kWarps * 32, smem, st>>>(a);
+    render_fwd_kernel<kWarps, kRays, kNV><<<grid, kWarps * 32, smem, st>>>(a);
     return IA_OK;
 }
 
-template <int kWarps, bool kKeepXc, bool kDynLanes = kKeepXc>
+template <int kWarps, bool kKeepXc, bool kDynLanes = kKeepXc, bool kNV = false>
 static int launch_query_t(QueryArgs& a, cudaStream_t stream) {
-    const size_t smem = sizeof(QuerySmem<kWarps, kKeepXc>);
+    const size_t smem = sizeof(QuerySmem<kWarps, kKeepXc, kNV>);
     static PerDeviceFlag attr_set;
     if (!attr_set.get()) {
-        IA_CHECK_CUDA(cudaFuncSetAttribute(deform_query_kernel<kWarps, kKeepXc, kDynLanes>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        IA_CHECK_CUDA(cudaFuncSetAttribute(deform_query_kernel<kWarps, kKeepXc, kDynLanes, kNV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set.set();
     }
     const int n_batches = a.grid_aabb ? (a.G * a.G * a.G + (32 / a.passes) - 1) / (32 / a.passes) : (a.n + 31) / 32;
     int grid = sm_count();
     if (grid <= 0) return set_err(IA_ECUDA, "no CUDA device%s");
     grid = min(grid, (n_batches + kWarps - 1) / kWarps);
-    deform_query_kernel<kWarps, kKeepXc, kDynLanes><<<grid, kWarps * 32, smem, stream>>>(a);
+    deform_query_kernel<kWarps, kKeepXc, kDynLanes, kNV><<<grid, kWarps * 32, smem, stream>>>(a);
     IA_CHECK_CUDA(cudaPeekAtLastError());
     return IA_OK;
 }
 
 static int launch_query(QueryArgs& a, cudaStream_t stream) {
+    if (a.sd.s.nv) {  // nearest-vertex deformer: one lane per point, default launch shape
+        a.lanes_per_sample = 1;
+        if (a.xc_best) return launch_query_t<12, true, false, true>(a, stream);
+        return launch_query_t<12, false, false, true>(a, stream);
+    }
     if (a.xc_best) return launch_query_t<12, true>(a, stream);
     if (a.grid_aabb && a.lanes_per_sample > 1) return launch_query_t<12, false, true>(a, stream);  // narrow occupancy batches
     switch (g_query_warps) {
@@ -1046,6 +1061,12 @@ static int render_fwd_impl(const IaScene* scene, const float* rays_o, const floa
     int* ws_cost = reinterpret_cast<int*>(reinterpret_cast<char*>(workspace) + 256);
     int* ws_order = ws_cost + (n_rays + 1);
     const int rpw = g_render_rays;
+    if (scene->nv) {  // nearest-vertex deformer: the default tile shape (results do not depend on it)
+        rc = launch_render<12, 4, true>(a, plan, ws_cost, ws_order, st);
+        if (rc) return rc;
+        IA_CHECK_CUDA(cudaPeekAtLastError());
+        return IA_OK;
+    }
     // (a 16-warp renderer no longer fits next to the staged hash level)
     switch (rpw) {
         case 32: rc = launch_render<12, 32>(a, plan, ws_cost, ws_order, st); break;
@@ -1071,6 +1092,7 @@ int ia_render_fwd_peer(const IaScene* scene, const float* rays_o, const float* r
                        int n_rays, const float* bg, int image_width, float* rgb, float* depth, float* alpha, float* counter,
                        void* workspace, size_t workspace_bytes, IaStats* stats, const int* pixel_index,
                        float* const* peer_rgba, int n_peers, ia_stream_t stream) {
+    IA_REJECT_NV(scene, "ia_render_fwd_peer");
     IA_REQUIRE(peer_rgba && n_peers >= 1 && n_peers <= 64);
     return render_fwd_impl(scene, rays_o, rays_d, near, far, n_rays, bg, image_width, rgb, depth, alpha, counter, workspace,
                            workspace_bytes, stats, pixel_index, peer_rgba, n_peers, stream);
@@ -1153,6 +1175,7 @@ extern "C" int ia_occupancy_query(const IaScene* scene, const float* jitter, con
 extern "C" int ia_occupancy_query_peer(const IaScene* scene, const float* jitter, const float* aabb, int G, int passes,
                                        float* const* peer_density, int n_peers, void* workspace, int shard, int n_shards,
                                        IaStats* stats, ia_stream_t stream) {
+    IA_REJECT_NV(scene, "ia_occupancy_query_peer");
     IA_REQUIRE(peer_density && n_peers >= 1 && n_peers <= 64);
     return occupancy_query_impl(scene, jitter, aabb, G, passes, nullptr, peer_density, n_peers, workspace, shard, n_shards, stats, stream);
 }
@@ -1162,12 +1185,14 @@ extern "C" int ia_occupancy_query_ordered(const IaScene* scene, const float* jit
                                           int shard, int n_shards, const int* batch_order, int n_order,
                                           unsigned* batch_cost, IaStats* stats, ia_stream_t stream) {
     IA_REQUIRE((density_max != nullptr) != (peer_density != nullptr));
+    if (peer_density) IA_REJECT_NV(scene, "ia_occupancy_query_ordered over peer memory");
     IA_REQUIRE(!peer_density || (n_peers >= 1 && n_peers <= 64));
     return occupancy_query_impl(scene, jitter, aabb, G, passes, density_max, peer_density, n_peers, workspace, shard, n_shards,
                                 stats, stream, batch_order, n_order, batch_cost);
 }
 
 int ia_broyden(const IaScene* scene, const float* xd, int n, float* xc, uint8_t* valid, float* j_inv, ia_stream_t stream) {
+    IA_REJECT_NV(scene, "ia_broyden");
     IA_REQUIRE(n >= 0);
     if (n == 0) return IA_OK;
     IA_REQUIRE(xd && xc && valid);

@@ -36,17 +36,22 @@ struct SceneDev {
     IaScene s;
     HashLevels hl;
     float filter_thr;
+    NvDev nv;   // valid when s.nv is set (nearest-vertex deformer)
 };
 
+// kNV: nearest-vertex deformer -- the Fast-SNARF constants (bone transforms, Broyden parameters) are not read
+template <bool kNV = false>
 __device__ __forceinline__ void load_frame_const(FrameConst& fc, const SceneDev& sd) {
     const int tid = threadIdx.x;
-    if (tid < kNumInit * 12) {
+    if (!kNV && tid < kNumInit * 12) {
         const int i = tid / 12, e = tid % 12;
         fc.Tb[i][e] = sd.s.tfs[c_init_bones[i] * 16 + e];  // rows 0..2 of the 4x4
     }
     if (tid < 3) {
-        fc.bp.off[tid] = sd.s.offset_k[tid];
-        fc.bp.scl[tid] = sd.s.scale_k[tid];
+        if (!kNV) {
+            fc.bp.off[tid] = sd.s.offset_k[tid];
+            fc.bp.scl[tid] = sd.s.scale_k[tid];
+        }
         if (sd.s.net_center) {
             fc.net_center[tid] = sd.s.net_center[tid];
             fc.net_scale[tid] = sd.s.net_scale[tid];
@@ -66,11 +71,26 @@ __device__ __forceinline__ void load_frame_const(FrameConst& fc, const SceneDev&
 }
 
 
+int ia_nv_check(const IaNearestVertex* nv);  // ia_nearest.cu
+
+// entry points without a nearest-vertex form reject a scene that has one
+#define IA_REJECT_NV(scene, what)                                                                        \
+    do {                                                                                                 \
+        if ((scene) && (scene)->nv)                                                                      \
+            return ia_set_err(IA_EINVAL, "%s does not support the nearest-vertex deformer (scene->nv)", what); \
+    } while (0)
+
 static int make_scene_dev(const IaScene* s, SceneDev& sd, bool need_occ, bool need_net = true) {
     IA_REQUIRE(s != nullptr);
-    IA_REQUIRE(s->field && s->offset_k && s->scale_k && s->tfs);
+    if (s->nv) {
+        const int rc = ia_nv_check(s->nv);
+        if (rc) return rc;
+        sd.nv = make_nv_dev(*s->nv);
+    } else {
+        IA_REQUIRE(s->field && s->offset_k && s->scale_k && s->tfs);
+        IA_REQUIRE(s->D > 1 && s->H > 1 && s->W > 1);
+    }
     if (need_net) IA_REQUIRE(s->table_h && s->mlp_h && s->net_center && s->net_scale);
-    IA_REQUIRE(s->D > 1 && s->H > 1 && s->W > 1);
     if (need_occ) {
         IA_REQUIRE(s->occ_bits && s->occ_aabb);
         IA_REQUIRE(s->G == 64);

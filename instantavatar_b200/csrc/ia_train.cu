@@ -1336,6 +1336,62 @@ __global__ void __launch_bounds__(256) pose_grad_kernel(const __grid_constant__ 
         if (acc[i] != 0.f) atomicAdd(&a.grad_tfs[(i / 12) * 16 + (i % 12)], acc[i]);
 }
 
+// Nearest-vertex deformer (smpl_deformer.py:107-108, x_c = T_inv[v][:3,:3] x + T_inv[v][:3,3]): d loss / d T_inv[v][r][c]
+// = g_r [x, 1]_c with g = d loss / d x_c, and d loss / d x = T_inv[v][:3,:3]^T g, which reaches the ray of the sample
+// through x = z * d + o (raymarcher_acc.py:159): d loss / d o += d loss / d x, d loss / d d += z d loss / d x.  The
+// vertex is piecewise constant in x (the search carries no gradient, smpl_deformer.py:94-95).  A list sample is given as
+// (ray index, z); its posed point is recomputed as the forward generated it and the vertex is found again by the forward's
+// own search (same inputs, same code: bit-identical), so the forward saves nothing per sample beyond the SNARF path's state.
+struct NvPoseGradArgs {
+    SceneDev sd;
+    const float* rays_o; const float* rays_d; int n_rays;
+    const float* l_rz; const int8_t* best; const float* denc; const int* count; int capacity;
+    float* grad_table;   // [V][12], accumulated (+=)
+    float* grad_o; float* grad_d;   // [n_rays][3], accumulated (+=), nullable
+};
+
+__global__ void __launch_bounds__(256) nv_pose_grad_kernel(const __grid_constant__ NvPoseGradArgs a) {
+    __shared__ float cs[6];
+    if (threadIdx.x < 3) { cs[threadIdx.x] = a.sd.s.net_center[threadIdx.x]; cs[3 + threadIdx.x] = a.sd.s.net_scale[threadIdx.x]; }
+    __syncthreads();
+    const int count = min(*a.count, a.capacity);
+    const __half2* table = reinterpret_cast<const __half2*>(a.sd.s.table_h);
+    for (int p = blockIdx.x * blockDim.x + threadIdx.x; p < count; p += gridDim.x * blockDim.x) {
+        if (a.best[p] < 0) continue;
+        const int ray = (int)a.l_rz[p * 3];
+        const float z = a.l_rz[p * 3 + 1];
+        if (ray < 0 || ray >= a.n_rays) continue;
+        // z * d + o with separate mul / add, as the march (train_march_kernel) and ia_composite_bwd compute it
+        const float x0 = z * a.rays_d[ray * 3] + a.rays_o[ray * 3];
+        const float x1 = z * a.rays_d[ray * 3 + 1] + a.rays_o[ray * 3 + 1];
+        const float x2 = z * a.rays_d[ray * 3 + 2] + a.rays_o[ray * 3 + 2];
+        float d2;
+        const int v = nv_nearest(a.sd.nv, x0, x1, x2, d2);
+        if (v < 0) continue;
+        float xc[3], g[3];
+        nv_apply(a.sd.nv, v, x0, x1, x2, xc);
+        hash_input_grad(a.sd.hl, table, cs, cs + 3, xc, a.denc + (long)p * 32, g);
+        if (g[0] == 0.f && g[1] == 0.f && g[2] == 0.f) continue;
+        const float xh[4] = {x0, x1, x2, 1.f};
+        float* row = a.grad_table + (long)v * 12;
+        float gx[3] = {0.f, 0.f, 0.f};
+        const float4* trow = reinterpret_cast<const float4*>(a.sd.nv.table + (long)v * 12);
+#pragma unroll
+        for (int r = 0; r < 3; r++) {
+            const float4 t = __ldg(trow + r);
+            gx[0] += g[r] * t.x; gx[1] += g[r] * t.y; gx[2] += g[r] * t.z;
+            if (g[r] == 0.f) continue;
+#pragma unroll
+            for (int c = 0; c < 4; c++) atomicAdd(row + r * 4 + c, g[r] * xh[c]);
+        }
+#pragma unroll
+        for (int c = 0; c < 3; c++) {
+            if (a.grad_o) atomicAdd(a.grad_o + ray * 3 + c, gx[c]);
+            if (a.grad_d) atomicAdd(a.grad_d + ray * 3 + c, z * gx[c]);
+        }
+    }
+}
+
 }  // namespace
 
 namespace {
@@ -1370,6 +1426,7 @@ extern "C" int ia_ngp_input_grad(const IaScene* scene, const float* x, const flo
 
 extern "C" int ia_pose_grad(const IaScene* scene, const float* lbs_voxel, const float* xd, const int8_t* best,
                             const float* denc, const int* count, int capacity, float* grad_tfs, ia_stream_t stream) {
+    IA_REJECT_NV(scene, "ia_pose_grad (use ia_nv_pose_grad)");
     IA_REQUIRE(capacity >= 0);
     if (capacity == 0) return IA_OK;
     IA_REQUIRE(lbs_voxel && xd && best && denc && count && grad_tfs);
@@ -1381,6 +1438,26 @@ extern "C" int ia_pose_grad(const IaScene* scene, const float* lbs_voxel, const 
     if (sms <= 0) return set_err(IA_ECUDA, "no CUDA device%s");
     const int n_batches = (capacity + 31) / 32;
     pose_grad_kernel<<<min(sms * 2, (n_batches + 7) / 8), 256, 0, (cudaStream_t)stream>>>(a);
+    IA_CHECK_CUDA(cudaPeekAtLastError());
+    return IA_OK;
+}
+
+extern "C" int ia_nv_pose_grad(const IaScene* scene, const float* rays_o, const float* rays_d, int n_rays, const float* l_rz,
+                               const int8_t* best, const float* denc, const int* count, int capacity, float* grad_table,
+                               float* grad_rays_o, float* grad_rays_d, ia_stream_t stream) {
+    IA_REQUIRE(scene && scene->nv);
+    IA_REQUIRE(capacity >= 0 && n_rays >= 0 && n_rays <= (1 << 24));  // ray indices travel as exact floats
+    if (capacity == 0 || n_rays == 0) return IA_OK;
+    IA_REQUIRE(rays_o && rays_d && l_rz && best && denc && count && grad_table);
+    NvPoseGradArgs a;
+    int rc = make_scene_dev(scene, a.sd, false);
+    if (rc) return rc;
+    a.rays_o = rays_o; a.rays_d = rays_d; a.n_rays = n_rays;
+    a.l_rz = l_rz; a.best = best; a.denc = denc; a.count = count; a.capacity = capacity; a.grad_table = grad_table;
+    a.grad_o = grad_rays_o; a.grad_d = grad_rays_d;
+    const int sms = sm_count();
+    if (sms <= 0) return set_err(IA_ECUDA, "no CUDA device%s");
+    nv_pose_grad_kernel<<<min(sms * 8, (capacity + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a);
     IA_CHECK_CUDA(cudaPeekAtLastError());
     return IA_OK;
 }
@@ -1397,6 +1474,7 @@ int ia_train_fwd(const IaScene* scene, const float* rays_o, const float* rays_d,
                  int n_rays, const float* bg, const float* jitter, const float* noise, float* rgb, float* depth,
                  float* alpha, float* weights, float* s_sigma, float* s_rgb, float* s_xc, float* s_z, int* s_count,
                  int8_t* s_best, void* workspace, IaStats* stats, ia_stream_t stream) {
+    IA_REJECT_NV(scene, "ia_train_fwd (use ia_train_fwd_split)");
     IA_REQUIRE(n_rays >= 0);
     if (n_rays == 0) return IA_OK;
     IA_REQUIRE(rays_o && rays_d && near && far && rgb && depth && alpha && weights && workspace);

@@ -9,6 +9,7 @@
 //   -> per-sample arg-max over the 13 candidates.
 #pragma once
 #include "ia_device.cuh"
+#include "ia_nv.cuh"
 
 namespace ia {
 
@@ -41,6 +42,13 @@ struct EvalCtx {
     const __half* Wsm;        // padded fp16 weights in shared memory
     const FrameConst* fc;     // shared memory
     const HashLevels* hl;     // kernel-parameter (constant bank) copy
+};
+
+// scratch of the nearest-vertex stage: one candidate per sample, so no 13-candidate arrays
+struct WarpScratchNV {
+    float cx[3][32];  // canonical points of the compacted valid samples
+    __align__(16) __half At[32][kW1Stride];
+    float res[32][4];
 };
 
 __device__ __forceinline__ int warp_excl_scan(int v, int lane, int& total) {
@@ -176,6 +184,62 @@ __device__ __forceinline__ void warp_eval_samples(const EvalCtx& ctx, WarpScratc
         out.best = best;
         if constexpr (kKeepXc) {
             out.xc[0] = ws.cand[0][best][lane]; out.xc[1] = ws.cand[1][best][lane]; out.xc[2] = ws.cand[2][best][lane];
+        }
+    }
+    __syncwarp();
+}
+
+// The same pipeline for the nearest-vertex deformer (smpl_deformer.py:87-137), one candidate per lane: grid search
+// (ia_nv.cuh) -> gathered affine -> compaction of the valid samples -> hash encode -> mlp_tile16 -> outputs.
+// Invalid samples: sigma = 0 (eval) / -1e5 (train), rgb = 0, best = -1.  At train time a valid sample whose network
+// output is not finite is invalid too (smpl_deformer.py:119-122); eval outputs are passed through as the reference does.
+// best = 0 marks a valid sample, so the training state and ia_composite_bwd's list compaction are the SNARF path's.
+__device__ __forceinline__ void warp_eval_nv(const EvalCtx& ctx, const NvDev& nv, WarpScratchNV& ws, bool active, float xd0,
+                                             float xd1, float xd2, bool eval_mode, int lane, SampleOut& out,
+                                             unsigned& nroots, unsigned& nhash) {
+    const FrameConst& fc = *ctx.fc;
+    bool valid = false;
+    float xc[3] = {0.f, 0.f, 0.f};
+    if (active) {
+        float d2;
+        const int v = nv_nearest(nv, xd0, xd1, xd2, d2);
+        if (v >= 0) {
+            nv_apply(nv, v, xd0, xd1, xd2, xc);
+            valid = true;
+        }
+    }
+    const unsigned vm = __ballot_sync(kFull, valid);
+    const int total = __popc(vm);
+    const int pos = __popc(vm & ((1u << lane) - 1u));
+    if (valid) { ws.cx[0][pos] = xc[0]; ws.cx[1][pos] = xc[1]; ws.cx[2][pos] = xc[2]; }
+    nroots += valid ? 1u : 0u;
+    __syncwarp();
+    if (total > 0) {
+        const bool has = lane < total;
+        __half2* arow = reinterpret_cast<__half2*>(&ws.At[lane][0]);
+        if (has) {
+            // ngp.py:75,77: x = (x - center) / scale + 0.5 ; clamp [0,1]
+            const float n0 = fminf(fmaxf((ws.cx[0][lane] - fc.net_center[0]) / fc.net_scale[0] + 0.5f, 0.f), 1.f);
+            const float n1 = fminf(fmaxf((ws.cx[1][lane] - fc.net_center[1]) / fc.net_scale[1] + 0.5f, 0.f), 1.f);
+            const float n2 = fminf(fmaxf((ws.cx[2][lane] - fc.net_center[2]) / fc.net_scale[2] + 0.5f, 0.f), 1.f);
+#pragma unroll 4
+            for (int l = 0; l < kLevels; l++) arow[l] = hash_encode_level(ctx.table, *ctx.hl, l, n0, n1, n2, &nhash);
+        } else {
+#pragma unroll
+            for (int l = 0; l < kLevels; l++) arow[l] = __floats2half2_rn(0.f, 0.f);
+        }
+        __syncwarp();
+        mlp_tile16(&ws.At[0][0], ctx.Wsm, &ws.res[0], lane);
+        if (total > 16) mlp_tile16(&ws.At[16][0], ctx.Wsm, &ws.res[16], lane);
+        __syncwarp();
+    }
+    out.sigma = eval_mode ? 0.f : -1e5f; out.r = out.g = out.b = 0.f; out.best = -1;
+    out.xc[0] = out.xc[1] = out.xc[2] = 0.f;
+    if (valid) {
+        const float s = ws.res[pos][0], cr = ws.res[pos][1], cg = ws.res[pos][2], cb = ws.res[pos][3];
+        if (eval_mode || (isfinite(s) && isfinite(cr) && isfinite(cg) && isfinite(cb))) {
+            out.sigma = s; out.r = cr; out.g = cg; out.b = cb; out.best = 0;
+            out.xc[0] = xc[0]; out.xc[1] = xc[1]; out.xc[2] = xc[2];
         }
     }
     __syncwarp();

@@ -6,6 +6,10 @@ are assembled once (batched 3x4 `rot` / `shift` tables, blend-shape offsets remo
 smpl_deformer.py:60-76); per sample the search is `ia_knn1` (pytorch3d knn_points K = 1 contract) and the transform is one
 gathered batched product.  The network is any `model(points, None)` callable; `NeRFNGPNet.forward` is differentiable
 w.r.t. parameters and points, so pose gradients flow through the gathered tables.
+
+With a NeRFNGPNet and one frame per batch, `scene()` hands the fused kernels (render, occupancy query, split training
+forward) a per-frame vertex bucket grid (`ia_nv_grid_build`) and the [V,12] table of T_inv rows instead of the Fast-SNARF
+field; `ia_nv_pose_grad` returns d loss / d table, which autograd carries back to the SMPL parameters.
 """
 from __future__ import annotations
 
@@ -33,6 +37,9 @@ class SMPLDeformer:
         self.body_model = SMPL(model_path, gender=gender, data_struct=smpl_data)
         self.k, self.threshold, self.strategy = k, threshold, "nearest_neighbor"
         self.initialized = False  # the reference re-initialises every frame (betas may be optimised); kept
+        self._nv = None       # this frame's ops.NearestVertex (built by scene(); owns its grid workspace, so a Scene kept for
+                              # a later backward keeps searching the frame it was made for)
+        self.nv_table = None  # [V,12] rows of T_inv[:3,:4] with their autograd history (the fused path's pose leaf)
 
     # ---- canonical template ------------------------------------------------------------------------
     def initialize(self, betas, device):
@@ -59,12 +66,40 @@ class SMPLDeformer:
         self.T_inv = self.T_template @ torch.cat([unpose, bottom], dim=-2)
         self.rot, self.shift = self.T_inv[..., :3, :3], self.T_inv[..., :3, 3]
         self.vertices = torch.baddbmm(self.w2s[:, None, :3, 3], posed.vertices, self.w2s[:, :3, :3].transpose(1, 2))
+        self._nv = None
 
     def get_bbox_deformed(self):
         return get_bbox_from_smpl(self.vertices[0:1].detach())
 
     def transform_rays_w2s(self, rays):
         rays_to_root_frame(rays, self.w2s)
+
+    # ---- fused kernels ------------------------------------------------------------------------------
+    def nearest_vertex(self) -> ops.NearestVertex:
+        """this frame's nearest-vertex state for the fused kernels: the bucket grid of the posed vertices and the contiguous
+        [V,12] table of T_inv rows, built on first use after prepare_deformer (which also runs on CPU tensors)"""
+        if not self.fusable:
+            raise NotImplementedError("SMPLDeformer on the fused kernels: one prepared frame per batch (the operator path serves batches)")
+        if self._nv is None:
+            table = self.T_inv[0, :, :3, :4].float().reshape(-1, 12).contiguous()
+            nv = ops.NearestVertex(verts=self.vertices[0].detach().float().contiguous(), table=table.detach(),
+                                   threshold=float(self.threshold))
+            self._nv = ops.nv_grid_build(nv)
+            self.nv_table = table
+        return self._nv
+
+    @property
+    def fusable(self) -> bool:
+        """True when the fused kernels can serve this deformer: prepare_deformer has run for exactly one frame"""
+        vertices = getattr(self, "vertices", None)
+        return vertices is not None and vertices.shape[0] == 1
+
+    def scene(self, net, occ_bits=None, occ_aabb=None) -> ops.Scene:
+        """the per-frame read-only state handed to the fused kernels"""
+        table_h, mlp_h = net.half_params()
+        return ops.Scene(table_h=table_h, mlp_h=mlp_h, net_center=net.center.reshape(3).contiguous().float(),
+                         net_scale=net.scale.reshape(3).contiguous().float(), occ_bits=occ_bits, occ_aabb=occ_aabb,
+                         nv=self.nearest_vertex())
 
     # ---- per sample ---------------------------------------------------------------------------------
     def deform(self, pts):

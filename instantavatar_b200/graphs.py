@@ -13,6 +13,14 @@ import torch
 RAY_KEYS = ("rays_o", "rays_d", "near", "far", "bg_color")
 
 
+def _require_graphable(model, what):
+    """the captured sequences are those of the Fast-SNARF deformer; the nearest-vertex deformer is not captured"""
+    from .deformers.smpl_deformer import SMPLDeformer
+    if isinstance(model.deformer, SMPLDeformer):
+        raise NotImplementedError(f"{what}: CUDA-graph capture is not implemented for the nearest-vertex deformer "
+                                  "(SMPLDeformer); call the model directly")
+
+
 class GraphedFrame:
     """render_image_fast on static input/output buffers.
 
@@ -22,6 +30,7 @@ class GraphedFrame:
     the large inputs is hidden behind work that does not read them."""
 
     def __init__(self, model, batch: dict, img_size, warmup: int = 3, jitters=None):
+        _require_graphable(model, "GraphedFrame")
         self.model, self.img_size = model, img_size
         self.static_in = {k: v.clone() for k, v in batch.items() if torch.is_tensor(v)}
         # the small per-frame inputs (SMPL pose: betas, global_orient, body_pose, transl, ...) live in ONE device buffer fed by
@@ -113,6 +122,7 @@ class GraphedTrainStep:
     refresh, with / without density noise), selected on the host from the step number -- no device read-back."""
 
     def __init__(self, model, batch: dict, warmup: int = 3):
+        _require_graphable(model, "GraphedTrainStep")
         self.model = model
         self.static_in = {k: v.clone() for k, v in batch.items() if torch.is_tensor(v)}
         self.graphs = {}
@@ -195,6 +205,7 @@ class GraphedShardedFrame:
     """DNeRFModel.render_image_sharded (one frame over several GPUs, two collectives) captured once per rank"""
 
     def __init__(self, model, batch: dict, img_size, rank, world, jitters, tile=2048, warmup=3, peer=None):
+        _require_graphable(model, "GraphedShardedFrame")
         self.static_in = {k: v.clone() for k, v in batch.items() if torch.is_tensor(v)}
         self.jitters = jitters.clone()
         model.eval()

@@ -9,6 +9,7 @@ from dataclasses import dataclass
 import torch
 
 from .. import ops
+from ..deformers.smpl_deformer import SMPLDeformer
 from ..deformers.snarf_deformer import SNARFDeformer
 from ..renderers.raymarcher_acc import BoundModel, Raymarcher
 from .networks.ngp import NeRFNGPNet
@@ -103,7 +104,10 @@ class DNeRFModel(torch.nn.Module):
         from .structures.body_model_param import SMPLParamEmbedding
         dev = self.net_coarse.encoder.params.device
         self.SMPL_param = SMPLParamEmbedding(**{k: torch.as_tensor(v) for k, v in smpl_params.items()}).to(dev)
-        group = [p for n, p in self.SMPL_param.named_parameters() if not n.startswith("betas")]
+        # DNeRF.py:39-40 puts every SMPL_param parameter in the group; the SNARF path never reads the optimised betas (its
+        # skinning field is built from the first frame's), so there they stay out.  SMPLDeformer re-poses with them.
+        with_betas = isinstance(self.deformer, SMPLDeformer)
+        group = [p for n, p in self.SMPL_param.named_parameters() if with_betas or not n.startswith("betas")]
         from ..optim import DeviceAdam
         self.pose_optimizer = DeviceAdam(group, lr=lr, betas=self.optimizer.betas, eps=self.optimizer.eps)
         self.pose_optimizer.set_lr_factor(self.optimizer.lr_factor)
@@ -182,10 +186,12 @@ class DNeRFModel(torch.nn.Module):
             # steps whose only pose-dependent loss is the ray loss (all steps when refining, else those without the grid
             # regulariser) run without an autograd graph: ia_pose_grad -> ia_smpl_tfs_backward -> index_add_ into the
             # embedding gradients; the whole step is then a fixed launch sequence (CUDA-graph capturable)
-            manual_pose = self.fused_loss and self.deformer.fast_prepare and (self.is_refine or self.global_step % 20 != 0)
+            manual_pose = (self.fused_loss and getattr(self.deformer, "fast_prepare", False)
+                           and (self.is_refine or self.global_step % 20 != 0))
             with torch.set_grad_enabled(not manual_pose):
                 body = self.SMPL_param(idx)
-            for k in ("global_orient", "body_pose", "transl"):
+            # DNeRF.py:121-123: the nearest-vertex deformer also takes the (optimised) shape
+            for k in ("global_orient", "body_pose", "transl") + (("betas",) if isinstance(self.deformer, SMPLDeformer) else ()):
                 batch[k] = body[k]
             cam_dist = torch.norm(batch["transl"], dim=-1, keepdim=True).detach()
             batch["near"] = torch.zeros_like(batch["near"]) + cam_dist - 1
@@ -216,8 +222,25 @@ class DNeRFModel(torch.nn.Module):
             losses, g_rgb, g_alpha, g_w = ops.nerf_loss(out, batch["rgb"], batch["alpha"], self.loss_fn.w_rgb, self.loss_fn.w_alpha,
                                                         self.loss_fn.w_reg, self.scaler.scale_t)
             from ..autograd import GRAD_SCALE
-            tfs = self.deformer.tfs
-            if tfs.requires_grad or manual_pose:
+            nv_leaves = [t for t in (self.deformer.nv_table, rays.o, rays.d) if t.requires_grad] if scene.nv is not None else []
+            if nv_leaves:
+                # nearest-vertex deformer: d loss / d T_inv table (body pose, shape) and d loss / d root-frame rays (their w2s
+                # carries the global rotation and translation, smpl_deformer.py:78-85), handed to autograd
+                l_xc, l_ds, l_dc, l_count, l_rz, l_best = ops.composite_bwd(near, far, bg, noise_tensor, saved, g_rgb, None, g_alpha, g_w,
+                                                                            rays=ops.ray_slot_codes(n, o.device))
+                denc = torch.empty((l_xc.shape[0], 32), device=o.device, dtype=torch.float32)
+                frozen = self.network_frozen
+                ops.ngp_backward(scene, l_xc, l_ds, l_dc, l_count, None if frozen else g_enc, None if frozen else g_col, GRAD_SCALE, denc)
+                g_table, g_o, g_d = torch.zeros_like(self.deformer.nv_table), torch.zeros_like(o), torch.zeros_like(d)
+                ops.nv_pose_grad(scene, o, d, l_rz, l_best, denc, l_count, g_table, g_o, g_d)
+                grads = {id(self.deformer.nv_table): g_table, id(rays.o): g_o.reshape(rays.o.shape), id(rays.d): g_d.reshape(rays.d.shape)}
+                torch.autograd.backward(nv_leaves, [grads[id(t)] for t in nv_leaves], retain_graph=reg is not None)
+            elif scene.nv is not None:
+                if not self.network_frozen:
+                    l_xc, l_ds, l_dc, l_count = ops.composite_bwd(near, far, bg, noise_tensor, saved, g_rgb, None, g_alpha, g_w)
+                    ops.ngp_backward(scene, l_xc, l_ds, l_dc, l_count, g_enc, g_col, GRAD_SCALE)
+            elif self.deformer.tfs.requires_grad or manual_pose:
+                tfs = self.deformer.tfs
                 # pose optimisation: d loss / d tfs by implicit differentiation of the roots (deformer_torch.py:50-67),
                 # handed to autograd at `tfs` so that the SMPL forward kinematics are differentiated by torch
                 l_xc, l_ds, l_dc, l_count, l_xd, l_best = ops.composite_bwd(near, far, bg, noise_tensor, saved, g_rgb, None, g_alpha, g_w,
@@ -283,6 +306,9 @@ class DNeRFModel(torch.nn.Module):
         peer (parallel.PeerFrame): both exchanges happen inside the kernels over NVLink peer memory (atomics into every
         rank's density grid, RGBA stores into every rank's image); the frame then needs two barriers and no collective."""
         from .. import parallel
+        if isinstance(self.deformer, SMPLDeformer):
+            raise NotImplementedError("render_image_sharded: the nearest-vertex deformer (SMPLDeformer) renders on one GPU; "
+                                      "use render_image_fast")
         H, W = img_size
         self.deformer.prepare_deformer(batch)
         self.net_coarse.initialize(self.deformer.bbox)

@@ -111,7 +111,7 @@ class DensityGrid(torch.nn.Module):
         symmetric density buffer, followed by one barrier."""
         self.aabb = deformer.get_bbox_deformed()
         from ..networks.ngp import NeRFNGPNet
-        if isinstance(net, NeRFNGPNet) and hasattr(deformer, "scene"):
+        if isinstance(net, NeRFNGPNet) and hasattr(deformer, "scene") and getattr(deformer, "fusable", True):
             # all passes in one launch of the fused point-query kernel (points generated from the cell index)
             if jitters is None:
                 jitters = torch.rand((iters, *self.coords.shape), device=self.coords.device)

@@ -8,7 +8,7 @@ from dataclasses import dataclass, field as dc_field
 import torch
 
 from . import _lib
-from ._lib import IaScene, IaStats, check, lib, ptr, stream
+from ._lib import IaNearestVertex, IaScene, IaStats, check, lib, ptr, stream
 
 f32 = torch.float32
 
@@ -108,8 +108,49 @@ def occupancy_query(scene, jitters: torch.Tensor, aabb6: torch.Tensor, density=N
 
 
 @dataclass
+class NearestVertex:
+    """Per-frame state of the nearest-vertex deformer (IaNearestVertex): posed vertices [V,3] in the root frame, the
+    [V,12] table of T_inv[:3,:4] rows, the threshold and the bucket-grid workspace (filled by nv_grid_build)."""
+    verts: torch.Tensor
+    table: torch.Tensor
+    threshold: float
+    grid: torch.Tensor | None = None
+
+    def c_struct(self) -> IaNearestVertex:
+        s = IaNearestVertex()
+        s.grid = ptr(self.grid).value; s.verts = ptr(self.verts, f32).value; s.table = ptr(self.table, f32).value
+        s.n_verts = self.verts.shape[0]; s.threshold = float(self.threshold)
+        return s
+
+
+def nv_workspace_bytes(n_verts: int) -> int:
+    return int(lib().ia_nv_workspace_bytes(C.c_int(n_verts)))
+
+
+def nv_grid_build(nv: NearestVertex) -> NearestVertex:
+    """bucket the posed vertices into nv.grid (allocated here when missing); no host synchronisation"""
+    nbytes = nv_workspace_bytes(nv.verts.shape[0])
+    if nv.grid is None or nv.grid.numel() < nbytes:
+        nv.grid = torch.empty(nbytes, device=nv.verts.device, dtype=torch.uint8)
+    s = nv.c_struct()
+    _lib.count(1); check(lib().ia_nv_grid_build(C.byref(s), stream()))
+    return nv
+
+
+def nv_nearest(nv: NearestVertex, pts):
+    """grid search of the nearest vertex within the threshold -> (dist_sq [n], idx [n] int64); -1 / inf where none"""
+    pts = pts.reshape(-1, 3).float().contiguous()
+    n = pts.shape[0]
+    idx = torch.empty(n, device=pts.device, dtype=torch.int32); d2 = torch.empty(n, device=pts.device, dtype=f32)
+    s = nv.c_struct()
+    _lib.count(1); check(lib().ia_nv_nearest(C.byref(s), ptr(pts, f32), C.c_int(n), ptr(idx, torch.int32), ptr(d2), stream()))
+    return d2, idx.long()
+
+
+@dataclass
 class Scene:
-    """Per-frame read-only state (IaScene) with the tensors that keep it alive."""
+    """Per-frame read-only state (IaScene) with the tensors that keep it alive.  `nv` set: nearest-vertex deformer
+    (the Fast-SNARF fields are not used)."""
     field: torch.Tensor | None = None     # [D,H,W,24]
     offset_k: torch.Tensor | None = None  # [3]
     scale_k: torch.Tensor | None = None   # [3]
@@ -121,6 +162,7 @@ class Scene:
     occ_bits: torch.Tensor | None = None
     occ_aabb: torch.Tensor | None = None   # [6]
     G: int = 64
+    nv: NearestVertex | None = None
     _keep: list = dc_field(default_factory=list)
 
     def c_struct(self) -> IaScene:
@@ -136,6 +178,8 @@ class Scene:
         s.table_h = ptr(self.table_h).value if self.table_h is not None else None
         s.mlp_h = ptr(self.mlp_h).value if self.mlp_h is not None else None
         s.net_center = o(self.net_center); s.net_scale = o(self.net_scale)
+        if self.nv is not None:
+            s.nv = C.pointer(self.nv.c_struct())   # the pointer object keeps the struct alive as long as `s`
         return s
 
 
@@ -455,6 +499,32 @@ def pose_grad(scene: Scene, lbs_voxel, xd, best, denc, count, grad_tfs):
                                             ptr(best, torch.int8), ptr(denc, f32), ptr(count), C.c_int(xd.shape[0]), ptr(grad_tfs, f32), stream()))
 
 
+_RAY_SLOT_CODES: dict = {}
+
+
+def ray_slot_codes(n_rays: int, device):
+    """rays (o_i = (i, 0, 0), d_i = (0, 1, 0)) for which ia_composite_bwd's l_xd output is (ray index, z, 0) per list
+    sample, exactly -- the list form ia_nv_pose_grad reads (cached per size and device)"""
+    key = (n_rays, str(device))
+    codes = _RAY_SLOT_CODES.get(key)
+    if codes is None:
+        o = torch.zeros((n_rays, 3), device=device, dtype=f32)
+        o[:, 0] = torch.arange(n_rays, device=device, dtype=f32)
+        d = torch.zeros((n_rays, 3), device=device, dtype=f32)
+        d[:, 1] = 1.0
+        codes = _RAY_SLOT_CODES[key] = (o, d)
+    return codes
+
+
+def nv_pose_grad(scene: Scene, rays_o, rays_d, l_rz, best, denc, count, grad_table, grad_rays_o=None, grad_rays_d=None):
+    """d loss / d nearest-vertex table [V,12] and, when given, d loss / d rays_o / rays_d [n,3] (all +=) for a
+    compositing-backward list whose l_xd was produced with ray_slot_codes (ia_nv_pose_grad)"""
+    n = rays_o.numel() // 3
+    _lib.count(1); check(lib().ia_nv_pose_grad(C.byref(scene.c_struct()), ptr(rays_o, f32), ptr(rays_d, f32), C.c_int(n), ptr(l_rz, f32),
+                                               ptr(best, torch.int8), ptr(denc, f32), ptr(count), C.c_int(l_rz.shape[0]),
+                                               ptr(grad_table, f32), ptr(grad_rays_o, f32), ptr(grad_rays_d, f32), stream()))
+
+
 def voxelize_weights(verts, vert_weights, xs, ys, zs, offset, scale, ratio, knn=30, smooth_passes=30):
     """query_weights_smpl (deformer_torch.py:225-244) -> lbs_voxel [1,24,D,H,W]"""
     dev = verts.device
@@ -555,6 +625,9 @@ def _device_of(args, kwargs):
         if torch.is_tensor(a):
             if a.is_cuda:
                 return a.device
+        elif isinstance(a, NearestVertex):
+            if a.verts.is_cuda:
+                return a.verts.device
         elif isinstance(a, Scene):
             for t in (a.field, a.table_h, a.tfs, a.occ_bits):
                 if t is not None and t.is_cuda:
@@ -581,6 +654,6 @@ def _on_device(fn):
 
 for _name, _fn in list(globals().items()):
     if callable(_fn) and getattr(_fn, "__module__", None) == __name__ and not _name.startswith("_") \
-            and _name not in ("Scene", "set_option", "new_stats", "stats_dict", "gather_ceiling") and isinstance(_fn, type(_on_device)):
+            and _name not in ("Scene", "NearestVertex", "set_option", "new_stats", "stats_dict", "gather_ceiling") and isinstance(_fn, type(_on_device)):
         globals()[_name] = _on_device(_fn)
 del _name, _fn

@@ -4,7 +4,8 @@ Same constructor, `initialize(N)`, `__call__(rays, model, eval_mode, noise, bg_c
 reference.  When `model` is bound to a SNARFDeformer + NeRFNGPNet pair (a `BoundModel`, or the reference's
 `lambda x, _: self.deformer(x, self.net_coarse, eval_mode)` closure) the whole per-ray path -- occupancy-grid march,
 Broyden root finding, hash grid + MLPs, compositing -- runs as one fused kernel (`ia_render_fwd`, and the
-`ia_train_fwd/bwd` pair for training) instead of the reference's host-synchronous window loop.
+`ia_train_fwd/bwd` pair for training) instead of the reference's host-synchronous window loop.  An SMPLDeformer (one
+frame) + NeRFNGPNet pair runs the same kernels with the nearest-vertex deform stage.
 """
 from __future__ import annotations
 
@@ -25,8 +26,9 @@ class BoundModel:
 
 
 def _unwrap(model):
-    """find (deformer, net) behind a model callable; None if it is not a SNARFDeformer + NeRFNGPNet pair (the fused
-    kernels implement exactly that pair; anything else goes through the kernel-for-kernel legacy path)"""
+    """find (deformer, net) behind a model callable; None unless it is a SNARFDeformer + NeRFNGPNet pair or a one-frame
+    SMPLDeformer + NeRFNGPNet pair (the pairs the fused kernels implement; anything else goes through the
+    kernel-for-kernel legacy path)"""
     pair = None
     if hasattr(model, "deformer") and hasattr(model, "net"):
         pair = (model.deformer, model.net)
@@ -37,6 +39,8 @@ def _unwrap(model):
                 pair = (obj.deformer, obj.net_coarse)
                 break
     if pair is None or not hasattr(pair[0], "scene") or not hasattr(pair[1], "half_params"):
+        return None
+    if not getattr(pair[0], "fusable", True):   # e.g. an SMPLDeformer prepared for several frames
         return None
     return pair
 
