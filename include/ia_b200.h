@@ -363,6 +363,22 @@ int ia_nerf_loss(int n_rays, int n_samples, const float* rgb, const float* alpha
                  const float* target_rgb, const float* target_alpha, float w_rgb, float w_alpha, float w_reg,
                  const float* scale_dev, float* g_rgb, float* g_alpha, float* g_weights, float* sums, ia_stream_t stream);
 
+/* NGPLoss forward + analytic backward (instant_avatar/utils/loss.py:8-51) on patch-major rays: patch p holds rays
+ * [p * patch_rays, (p + 1) * patch_rays) ([B, P, h, w] flattened, patch_rays = h * w; n_rays % patch_rays != 0 ->
+ * IA_EINVAL).  NeRFLoss's terms give the same per-element gradients as ia_nerf_loss, bit for bit.  Added:
+ *   depth-variance regulariser  L_d = (1/N) sum_i a_i |d_i - mu_p|,  mu_p = sum_p d a / S_p,  S_p = sum_p a + 1e-3,
+ *   N = n_rays, weighted by w_depth_reg; with s_i = sign(d_i - mu_p) (0 at equality) and K_p = sum_p a s:
+ *   dL_d/dd_i = (a_i s_i - K_p a_i / S_p) / N,  dL_d/da_i = (|d_i - mu_p| - K_p (d_i - mu_p) / S_p) / N.
+ *   Each patch is reduced by one CTA in a fixed order: g_depth and g_alpha are the same in every run.
+ *   g_rgb_extra [n_rays][3] (nullable): a further d loss / d rgb (the LPIPS term, evaluated by the caller), added to g_rgb.
+ * All gradients are multiplied by *scale_dev (NULL = 1).  g_depth is written (zero when w_depth_reg == 0).
+ * sums [16] (zeroed by the library): ia_nerf_loss's layout ([0..3] sums, [4..8] terms, [8] = NeRFLoss total, [11] block
+ * ticket) plus [9] = sum a |d - mu|, [10] = loss_depth_reg, [12] = NeRFLoss total + w_depth_reg * loss_depth_reg. */
+int ia_ngp_loss(int n_rays, int n_samples, int patch_rays, const float* rgb, const float* alpha, const float* depth,
+                const float* weights, const float* target_rgb, const float* target_alpha, float w_rgb, float w_alpha,
+                float w_reg, float w_depth_reg, const float* g_rgb_extra /*nullable*/, const float* scale_dev /*nullable*/,
+                float* g_rgb, float* g_alpha, float* g_depth, float* g_weights, float* sums, ia_stream_t stream);
+
 /* Fused dense Adam (torch.optim.Adam semantics, models/DNeRF.py:46-50) on a flat fp32 tensor; gradients are
  * multiplied by inv_grad_scale (GradScaler unscale, DNeRF.py:157-158); if found_inf (device, nullable) is non-zero
  * the step is skipped.  ia_grad_check_finite sets *found_inf = 1 when any gradient is non-finite. */

@@ -1770,6 +1770,71 @@ __device__ __forceinline__ void reg_term(float x, float& val, float& dval) {
     dval = (a - b) / (a + b);
 }
 
+// NeRFLoss terms of one sample weight: g_weights[i] = d loss / d w times scale (gw = scale * w_reg / total); returns reg(w)
+// for the sums.  Shared by nerf_loss_kernel and ngp_loss_kernel, so both give bit-identical per-element gradients.
+__device__ __forceinline__ float nerf_weight_elem(long i, const float* __restrict__ weights, float gw, float* __restrict__ g_weights) {
+    float v, dv;
+    reg_term(weights[i], v, dv);
+    g_weights[i] = dv * gw;
+    return v;
+}
+
+// NeRFLoss terms of ray r: g_rgb[r][:] = d loss / d rgb (plus g_rgb_extra[r][:] when given), the return value is
+// d loss / d alpha (all times scale); the ray's (rgb-t)^2, (alpha-a)^2 and reg(alpha) are added to the running sums
+__device__ __forceinline__ float nerf_ray_elem(long r, int n_rays, const float* __restrict__ rgb, const float* __restrict__ alpha,
+                                               const float* __restrict__ t_rgb, const float* __restrict__ t_alpha, float w_rgb,
+                                               float w_alpha, float w_reg, float scale, const float* __restrict__ g_rgb_extra,
+                                               float* __restrict__ g_rgb, float& s_rgb, float& s_a, float& s_ra) {
+    for (int c = 0; c < 3; c++) {
+        const float d = rgb[r * 3 + c] - t_rgb[r * 3 + c];
+        s_rgb += d * d;
+        float g = scale * w_rgb * 2.f * d / (float)(n_rays * 3);
+        if (g_rgb_extra) g += g_rgb_extra[r * 3 + c] * scale;
+        g_rgb[r * 3 + c] = g;
+    }
+    const float da = alpha[r] - t_alpha[r];
+    s_a += da * da;
+    float v, dv;
+    reg_term(alpha[r], v, dv);
+    s_ra += v;
+    return scale * (w_alpha * 2.f * da / (float)n_rays + w_reg * dv / (float)n_rays);
+}
+
+// block reduction of K running sums, then ONE atomic per block and value (19 k same-address atomics would serialise at L2):
+// values 0..3 go to sums[0..3], value 4 to sums[9].  Returns true in the last block to finish (ticket in sums[11]).
+template <int K>
+__device__ __forceinline__ bool loss_sums_atomic(const float (&vals)[K], float* sums) {
+    __shared__ float red[8][K];
+    __shared__ bool last;
+#pragma unroll
+    for (int k = 0; k < K; k++) {
+        float v = vals[k];
+        for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+        if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5][k] = v;
+    }
+    __syncthreads();
+    if (threadIdx.x < K) {
+        float v = 0.f;
+        for (int w = 0; w < 8; w++) v += red[w][threadIdx.x];
+        atomicAdd(&sums[threadIdx.x < 4 ? threadIdx.x : 5 + threadIdx.x], v);
+    }
+    __threadfence();
+    __syncthreads();
+    if (threadIdx.x == 0) last = atomicAdd(reinterpret_cast<unsigned*>(sums) + 11, 1u) == gridDim.x - 1;
+    __syncthreads();
+    return last;
+}
+
+// the last block turns the four NeRFLoss sums into the loss terms the reference logs (loss.py:58-79), so no element-wise
+// torch launches follow: sums[4..8] = {mse_loss, loss_alpha_coarse, reg_alpha, reg_density, loss}
+__device__ __forceinline__ void nerf_loss_finish(float* sums, int n_rays, int S, float w_rgb, float w_alpha, float w_reg) {
+    const volatile float* sv = sums;
+    const float OFFSET = 0.313262f, n = (float)n_rays;
+    const float mse = sv[0] / (3.0f * n), msa = sv[1] / n, ra = sv[2] / n + OFFSET, rw = sv[3] / (n * (float)S) + OFFSET;
+    sums[4] = mse; sums[5] = msa; sums[6] = ra; sums[7] = rw;
+    sums[8] = ((w_rgb * mse + w_alpha * msa) + w_reg * ra) + w_reg * rw;
+}
+
 // out[0..4] += {sum (rgb-t)^2, sum (alpha-a)^2, sum reg(alpha), sum reg(w)} ; gradients of
 // loss = w_rgb mse_rgb + w_alpha mse_alpha + w_reg (mean reg(alpha) + mean reg(w)) (+ constants), times *scale
 __global__ void __launch_bounds__(256) nerf_loss_kernel(int n_rays, int S, const float* __restrict__ rgb, const float* __restrict__ alpha,
@@ -1781,52 +1846,89 @@ __global__ void __launch_bounds__(256) nerf_loss_kernel(int n_rays, int S, const
     const long total = (long)n_rays * S;
     float s_rgb = 0.f, s_a = 0.f, s_ra = 0.f, s_rw = 0.f;
     const float gw = scale * w_reg / (float)total;
-    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x) {
-        float v, dv;
-        reg_term(weights[i], v, dv);
-        s_rw += v;
-        g_weights[i] = dv * gw;
-    }
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x)
+        s_rw += nerf_weight_elem(i, weights, gw, g_weights);
     for (long r = (long)blockIdx.x * blockDim.x + threadIdx.x; r < n_rays; r += (long)gridDim.x * blockDim.x) {
-        for (int c = 0; c < 3; c++) {
-            const float d = rgb[r * 3 + c] - t_rgb[r * 3 + c];
-            s_rgb += d * d;
-            g_rgb[r * 3 + c] = scale * w_rgb * 2.f * d / (float)(n_rays * 3);
+        g_alpha[r] = nerf_ray_elem(r, n_rays, rgb, alpha, t_rgb, t_alpha, w_rgb, w_alpha, w_reg, scale, nullptr, g_rgb, s_rgb, s_a, s_ra);
+    }
+    const float vals[4] = {s_rgb, s_a, s_ra, s_rw};
+    if (loss_sums_atomic(vals, sums) && threadIdx.x == 0) nerf_loss_finish(sums, n_rays, S, w_rgb, w_alpha, w_reg);
+}
+
+// sum of two values over the block in a fixed order (same result in every thread and every run)
+__device__ __forceinline__ void block_sum2(float& a, float& b, float (*red)[2]) {
+    for (int o = 16; o; o >>= 1) {
+        a += __shfl_xor_sync(0xffffffffu, a, o);
+        b += __shfl_xor_sync(0xffffffffu, b, o);
+    }
+    if ((threadIdx.x & 31) == 0) { red[threadIdx.x >> 5][0] = a; red[threadIdx.x >> 5][1] = b; }
+    __syncthreads();
+    a = 0.f; b = 0.f;
+    for (int w = 0; w < 8; w++) { a += red[w][0]; b += red[w][1]; }
+    __syncthreads();   // red is reused by the next call
+}
+
+// NGPLoss (utils/loss.py:8-51) on patch-major rays: NeRFLoss's terms through the shared element helpers, the depth-variance
+// regulariser of each patch and an optional extra d loss / d rgb (the LPIPS term, computed by the caller).  Each patch is
+// reduced by ONE CTA in a fixed order, so g_depth and g_alpha do not depend on the run.
+__global__ void __launch_bounds__(256) ngp_loss_kernel(int n_rays, int S, int patch_rays, const float* __restrict__ rgb,
+                                                       const float* __restrict__ alpha, const float* __restrict__ depth,
+                                                       const float* __restrict__ weights, const float* __restrict__ t_rgb,
+                                                       const float* __restrict__ t_alpha, float w_rgb, float w_alpha, float w_reg,
+                                                       float w_depth_reg, const float* __restrict__ g_rgb_extra,
+                                                       const float* __restrict__ scale_dev, float* __restrict__ g_rgb,
+                                                       float* __restrict__ g_alpha, float* __restrict__ g_depth,
+                                                       float* __restrict__ g_weights, float* __restrict__ sums) {
+    __shared__ float red[8][2];
+    const float scale = scale_dev ? *scale_dev : 1.f;
+    const long total = (long)n_rays * S;
+    float s_rgb = 0.f, s_a = 0.f, s_ra = 0.f, s_rw = 0.f, s_dr = 0.f;
+    const float gw = scale * w_reg / (float)total;
+    for (long i = (long)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (long)gridDim.x * blockDim.x)
+        s_rw += nerf_weight_elem(i, weights, gw, g_weights);
+    const float gd = scale * w_depth_reg / (float)n_rays;
+    const int n_patches = n_rays / patch_rays;
+    for (int p = blockIdx.x; p < n_patches; p += gridDim.x) {
+        const long base = (long)p * patch_rays;
+        // mean depth of the patch: mu = sum d a / (sum a + 1e-3)
+        float sa = 0.f, sda = 0.f;
+        for (int j = threadIdx.x; j < patch_rays; j += blockDim.x) {
+            const float a = alpha[base + j];
+            sa += a;
+            sda += depth[base + j] * a;
         }
-        const float da = alpha[r] - t_alpha[r];
-        s_a += da * da;
-        float v, dv;
-        reg_term(alpha[r], v, dv);
-        s_ra += v;
-        g_alpha[r] = scale * (w_alpha * 2.f * da / (float)n_rays + w_reg * dv / (float)n_rays);
+        block_sum2(sa, sda, red);
+        const float sp = sa + 1e-3f, mu = sda / sp;
+        // K = sum a sign(d - mu) (sign 0 at d == mu, as torch's abs backward) and the patch's sum a |d - mu|
+        float kp = 0.f, l = 0.f;
+        for (int j = threadIdx.x; j < patch_rays; j += blockDim.x) {
+            const float a = alpha[base + j], diff = depth[base + j] - mu;
+            kp += a * (float)((diff > 0.f) - (diff < 0.f));
+            l += a * fabsf(diff);
+        }
+        block_sum2(kp, l, red);
+        if (threadIdx.x == 0) s_dr += l;
+        for (int j = threadIdx.x; j < patch_rays; j += blockDim.x) {
+            const long r = base + j;
+            float ga = nerf_ray_elem(r, n_rays, rgb, alpha, t_rgb, t_alpha, w_rgb, w_alpha, w_reg, scale, g_rgb_extra, g_rgb, s_rgb, s_a, s_ra);
+            float gdep = 0.f;
+            if (w_depth_reg != 0.f) {
+                // L_d = (1/N) sum a_i |d_i - mu|:  dL/dd_i = (a_i s_i - K a_i / S) / N,  dL/da_i = (|d_i - mu| - K (d_i - mu) / S) / N
+                const float a = alpha[r], diff = depth[r] - mu, s = (float)((diff > 0.f) - (diff < 0.f));
+                gdep = gd * (a * s - kp * a / sp);
+                ga += gd * (fabsf(diff) - kp * diff / sp);
+            }
+            g_alpha[r] = ga;
+            g_depth[r] = gdep;
+        }
     }
-    // block reduction, then ONE atomic per block and value (19 k same-address atomics would serialise at L2); the last block to finish turns the four sums into the loss terms the reference logs (loss.py:58-79), so no
-    // element-wise torch launches follow
-    float vals[4] = {s_rgb, s_a, s_ra, s_rw};
-    __shared__ float red[8][4];
-    __shared__ bool last;
-#pragma unroll
-    for (int k = 0; k < 4; k++) {
-        float v = vals[k];
-        for (int o = 16; o; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
-        if ((threadIdx.x & 31) == 0) red[threadIdx.x >> 5][k] = v;
-    }
-    __syncthreads();
-    if (threadIdx.x < 4) {
-        float v = 0.f;
-        for (int w = 0; w < 8; w++) v += red[w][threadIdx.x];
-        atomicAdd(&sums[threadIdx.x], v);
-    }
-    __threadfence();
-    __syncthreads();
-    if (threadIdx.x == 0) last = atomicAdd(reinterpret_cast<unsigned*>(sums) + 11, 1u) == gridDim.x - 1;
-    __syncthreads();
-    if (last && threadIdx.x == 0) {
+    const float vals[5] = {s_rgb, s_a, s_ra, s_rw, s_dr};
+    if (loss_sums_atomic(vals, sums) && threadIdx.x == 0) {
+        nerf_loss_finish(sums, n_rays, S, w_rgb, w_alpha, w_reg);
         const volatile float* sv = sums;
-        const float OFFSET = 0.313262f, n = (float)n_rays;
-        const float mse = sv[0] / (3.0f * n), msa = sv[1] / n, ra = sv[2] / n + OFFSET, rw = sv[3] / (n * (float)S) + OFFSET;
-        sums[4] = mse; sums[5] = msa; sums[6] = ra; sums[7] = rw;
-        sums[8] = ((w_rgb * mse + w_alpha * msa) + w_reg * ra) + w_reg * rw;
+        const float dr = sv[9] / (float)n_rays;
+        sums[10] = dr;
+        sums[12] = (((w_rgb * sv[4] + w_alpha * sv[5]) + w_depth_reg * dr) + w_reg * sv[6]) + w_reg * sv[7];
     }
 }
 
@@ -1843,6 +1945,22 @@ extern "C" int ia_nerf_loss(int n_rays, int n_samples, const float* rgb, const f
     const int sms = sm_count() > 0 ? sm_count() : 132;
     nerf_loss_kernel<<<sms * 4, 256, 0, st>>>(n_rays, n_samples, rgb, alpha, weights, target_rgb, target_alpha, w_rgb, w_alpha, w_reg,
                                               scale_dev, g_rgb, g_alpha, g_weights, sums);
+    IA_CHECK_CUDA(cudaPeekAtLastError());
+    return IA_OK;
+}
+
+extern "C" int ia_ngp_loss(int n_rays, int n_samples, int patch_rays, const float* rgb, const float* alpha, const float* depth,
+                           const float* weights, const float* target_rgb, const float* target_alpha, float w_rgb, float w_alpha,
+                           float w_reg, float w_depth_reg, const float* g_rgb_extra, const float* scale_dev, float* g_rgb,
+                           float* g_alpha, float* g_depth, float* g_weights, float* sums, ia_stream_t stream) {
+    IA_REQUIRE(n_rays > 0 && n_samples > 0 && patch_rays > 0 && n_rays % patch_rays == 0);
+    IA_REQUIRE(rgb && alpha && depth && weights && target_rgb && target_alpha && g_rgb && g_alpha && g_depth && g_weights && sums);
+    cudaStream_t st = (cudaStream_t)stream;
+    IA_CHECK_CUDA(cudaMemsetAsync(sums, 0, 16 * sizeof(float), st));
+    const int sms = sm_count() > 0 ? sm_count() : 132;
+    ngp_loss_kernel<<<sms * 4, 256, 0, st>>>(n_rays, n_samples, patch_rays, rgb, alpha, depth, weights, target_rgb, target_alpha,
+                                             w_rgb, w_alpha, w_reg, w_depth_reg, g_rgb_extra, scale_dev, g_rgb, g_alpha, g_depth,
+                                             g_weights, sums);
     IA_CHECK_CUDA(cudaPeekAtLastError());
     return IA_OK;
 }

@@ -33,13 +33,55 @@ def sharded_rays_per_warp(full_frame_rpw: int, world: int) -> int:
     return rpw
 
 
+def fused_loss_grads(loss_fn, out, batch, scale_dev=None, world_size=1):
+    """The loss of the fused training step and its gradients w.r.t. the per-ray outputs of ops.train_fwd, times the
+    GradScaler scale -> (losses, g_rgb, g_alpha, g_depth or None, g_weights).
+
+    An NGPLoss with a depth or LPIPS weight on a patch batch (`batch["rgb"]` of shape [B, P, h, w, 3], the reference's
+    `len(shape) == 5` rule, utils/loss.py:27,33) runs ops.ngp_loss: NeRFLoss's terms, the depth-variance regulariser of each
+    patch and the LPIPS term.  LPIPS is evaluated in torch on the rendered patches (its callable is the user's), and its
+    gradient w.r.t. the rendered colours is handed to the kernel.  The reference sums LPIPS over patches while the
+    multi-GPU step averages the summed gradients over `world_size` ranks, so that gradient is multiplied by `world_size`.
+    Everything else (NeRFLoss, an NGPLoss without patch weights, per-ray batches) runs ops.nerf_loss."""
+    from ..utils_loss import NGPLoss
+    tgt = batch["rgb"]
+    w_lpips = float(loss_fn.w_lpips) if isinstance(loss_fn, NGPLoss) else 0.0
+    w_depth = float(loss_fn.w_depth_reg) if isinstance(loss_fn, NGPLoss) else 0.0
+    if not ((w_lpips > 0 or w_depth > 0) and tgt.dim() == 5):
+        losses, g_rgb, g_alpha, g_w = ops.nerf_loss(out, tgt, batch["alpha"], loss_fn.w_rgb, loss_fn.w_alpha, loss_fn.w_reg, scale_dev)
+        return losses, g_rgb, g_alpha, None, g_w
+    B, P, h, w = tgt.shape[:4]
+    n = out["rgb"].shape[0]
+    if n % (h * w) != 0 or n != B * P * h * w:
+        raise ValueError(f"NGPLoss patch terms need whole {h}x{w} patches: {n} rays for a target of shape {tuple(tgt.shape)}"
+                         + (f" (with world_size {world_size} every rank's shard must hold whole patches)" if world_size > 1 else ""))
+    extra = lpips = None
+    if w_lpips > 0:
+        nchw = lambda t: t.flip(-1).flatten(0, 1).permute(0, 3, 1, 2)   # RGB -> BGR, [B*P, 3, h, w] (utils/loss.py:28-29)
+        with torch.enable_grad():
+            pred = out["rgb"].detach().reshape(tgt.shape).requires_grad_(True)
+            lpips = loss_fn.lpips(nchw(pred).clip(max=1), nchw(tgt.detach())).sum()
+            (g,) = torch.autograd.grad(lpips, pred)
+        extra = g.reshape(-1, 3) * (w_lpips * world_size)
+    losses, g_rgb, g_alpha, g_depth, g_w = ops.ngp_loss(out, tgt, batch["alpha"], h * w, loss_fn.w_rgb, loss_fn.w_alpha,
+                                                        loss_fn.w_reg, w_depth, extra, scale_dev)
+    if w_depth <= 0:   # NGPLoss logs the term only when it is weighted
+        del losses["loss_depth_reg"]
+        g_depth = None
+    if lpips is not None:
+        losses["loss_lpips"] = lpips.detach()
+        losses["loss"] = losses["loss"] + w_lpips * losses["loss_lpips"]
+    return losses, g_rgb, g_alpha, g_depth, g_w
+
+
 class DNeRFModel(torch.nn.Module):
     def __init__(self, opt=None, datamodule=None, smpl_data=None, model_path=None, gender="male", n_train_frames=1, device="cuda",
-                 net_seed=1337, deformer_opt=None):
+                 net_seed=1337, deformer_opt=None, lpips=None):
         """Two forms.  The reference's (DNeRF.py:18-30): `DNeRFModel(opt, datamodule)` with `opt` the `model.opt` node of
         confs/SNARF_NGP*.yaml (network / deformer / renderer / loss given as `_target_` configs, optimizer, scheduler,
         optimize_SMPL) and `datamodule.trainset` supplying `len()` and `get_SMPL_params()`.  Or keyword arguments only
-        (tests, bench): the SNARF_NGP.yaml defaults with a synthetic SMPL dictionary."""
+        (tests, bench): the SNARF_NGP.yaml defaults with a synthetic SMPL dictionary.  `lpips`: the LPIPS callable
+        `lpips(pred_nchw, target_nchw) -> [N,1,1,1]` handed to an NGPLoss config (the reference builds LPIPS-VGG itself)."""
         super().__init__()
         from ..optim import FusedAdam, GradScaler
         from ..utils_loss import NeRFLoss
@@ -50,7 +92,8 @@ class DNeRFModel(torch.nn.Module):
             opt = Cfg.wrap(dict(opt))
             self.net_coarse = instantiate(opt["network"]).to(device)
             self.deformer = instantiate(opt["deformer"], **({"smpl_data": smpl_data} if smpl_data is not None else {}))
-            self.loss_fn = instantiate(opt["loss"]) if "loss" in opt else NeRFLoss()
+            self.loss_fn = (instantiate(opt["loss"], **({"lpips": lpips} if lpips is not None else {})) if "loss" in opt
+                            else NeRFLoss())
             self.renderer = instantiate(opt["renderer"], smpl_init=opt.get("smpl_init", False), device=device)
             n_train_frames = len(datamodule.trainset) if datamodule is not None else n_train_frames
             o = opt.get("optimizer", {})
@@ -204,8 +247,8 @@ class DNeRFModel(torch.nn.Module):
         g_enc, g_col = self.net_coarse.grad_buffers()  # zeroed at creation and by every fused optimiser step
         reg = self.update_density_grid(grid_jitter)
         if self.fused_loss:
-            # forward kernel -> NeRFLoss forward+backward kernel -> compositing backward -> network backward: no autograd
-            # graph for the per-ray path (the grid regulariser below still goes through autograd, every 20 steps)
+            # forward kernel -> loss forward+backward kernel -> compositing backward -> network backward: no autograd
+            # graph for the per-ray path (the grid regulariser below, and an LPIPS term, still go through autograd)
             rays = Rays(o=batch["rays_o"], d=batch["rays_d"], near=batch["near"], far=batch["far"])
             self.deformer.transform_rays_w2s(rays)
             grid = self.renderer.density_grid_train
@@ -219,14 +262,13 @@ class DNeRFModel(torch.nn.Module):
                 noise_tensor = torch.randn((n, 256), device=near.device)
             bg = batch["bg_color"].reshape(-1, 3).float().contiguous() if batch.get("bg_color", None) is not None else None
             out, saved = ops.train_fwd(scene, o, d, near, far, bg, jitter, noise_tensor)
-            losses, g_rgb, g_alpha, g_w = ops.nerf_loss(out, batch["rgb"], batch["alpha"], self.loss_fn.w_rgb, self.loss_fn.w_alpha,
-                                                        self.loss_fn.w_reg, self.scaler.scale_t)
+            losses, g_rgb, g_alpha, g_depth, g_w = fused_loss_grads(self.loss_fn, out, batch, self.scaler.scale_t, self.world_size)
             from ..autograd import GRAD_SCALE
             nv_leaves = [t for t in (self.deformer.nv_table, rays.o, rays.d) if t.requires_grad] if scene.nv is not None else []
             if nv_leaves:
                 # nearest-vertex deformer: d loss / d T_inv table (body pose, shape) and d loss / d root-frame rays (their w2s
                 # carries the global rotation and translation, smpl_deformer.py:78-85), handed to autograd
-                l_xc, l_ds, l_dc, l_count, l_rz, l_best = ops.composite_bwd(near, far, bg, noise_tensor, saved, g_rgb, None, g_alpha, g_w,
+                l_xc, l_ds, l_dc, l_count, l_rz, l_best = ops.composite_bwd(near, far, bg, noise_tensor, saved, g_rgb, g_depth, g_alpha, g_w,
                                                                             rays=ops.ray_slot_codes(n, o.device))
                 denc = torch.empty((l_xc.shape[0], 32), device=o.device, dtype=torch.float32)
                 frozen = self.network_frozen
@@ -237,13 +279,13 @@ class DNeRFModel(torch.nn.Module):
                 torch.autograd.backward(nv_leaves, [grads[id(t)] for t in nv_leaves], retain_graph=reg is not None)
             elif scene.nv is not None:
                 if not self.network_frozen:
-                    l_xc, l_ds, l_dc, l_count = ops.composite_bwd(near, far, bg, noise_tensor, saved, g_rgb, None, g_alpha, g_w)
+                    l_xc, l_ds, l_dc, l_count = ops.composite_bwd(near, far, bg, noise_tensor, saved, g_rgb, g_depth, g_alpha, g_w)
                     ops.ngp_backward(scene, l_xc, l_ds, l_dc, l_count, g_enc, g_col, GRAD_SCALE)
             elif self.deformer.tfs.requires_grad or manual_pose:
                 tfs = self.deformer.tfs
                 # pose optimisation: d loss / d tfs by implicit differentiation of the roots (deformer_torch.py:50-67),
                 # handed to autograd at `tfs` so that the SMPL forward kinematics are differentiated by torch
-                l_xc, l_ds, l_dc, l_count, l_xd, l_best = ops.composite_bwd(near, far, bg, noise_tensor, saved, g_rgb, None, g_alpha, g_w,
+                l_xc, l_ds, l_dc, l_count, l_xd, l_best = ops.composite_bwd(near, far, bg, noise_tensor, saved, g_rgb, g_depth, g_alpha, g_w,
                                                                             rays=(o, d))
                 denc = torch.empty((l_xc.shape[0], 32), device=o.device, dtype=torch.float32)
                 frozen = self.network_frozen
@@ -262,7 +304,7 @@ class DNeRFModel(torch.nn.Module):
                 else:
                     tfs.backward(g_tfs.reshape(tfs.shape), retain_graph=reg is not None)
             elif not self.network_frozen:
-                l_xc, l_ds, l_dc, l_count = ops.composite_bwd(near, far, bg, noise_tensor, saved, g_rgb, None, g_alpha, g_w)
+                l_xc, l_ds, l_dc, l_count = ops.composite_bwd(near, far, bg, noise_tensor, saved, g_rgb, g_depth, g_alpha, g_w)
                 ops.ngp_backward(scene, l_xc, l_ds, l_dc, l_count, g_enc, g_col, GRAD_SCALE)
             if reg is not None and self.is_refine:  # DNeRF.py:139: the regulariser is dropped when refining poses
                 reg = None

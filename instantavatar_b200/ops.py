@@ -493,6 +493,28 @@ def nerf_loss(out: dict, target_rgb, target_alpha, w_rgb=1.0, w_alpha=0.1, w_reg
     return losses, g_rgb, g_alpha, g_w
 
 
+def ngp_loss(out: dict, target_rgb, target_alpha, patch_rays: int, w_rgb=1.0, w_alpha=0.1, w_reg=0.1, w_depth_reg=0.0,
+             g_rgb_extra=None, scale_dev=None):
+    """NGPLoss (utils/loss.py:8-51) forward + gradients w.r.t. (rgb, alpha, depth, weights) in one launch, on patch-major
+    rays (patch_rays = h * w of [B, P, h, w] patches).  g_rgb_extra [n, 3] (optional): a further d loss / d rgb -- the LPIPS
+    term's -- added to g_rgb.  Returns (losses dict of device scalars, g_rgb, g_alpha, g_depth, g_weights); `losses["loss"]`
+    holds the NeRFLoss terms and the depth regulariser."""
+    n, S = out["weights"].shape
+    dev = out["rgb"].device
+    g_rgb = torch.empty_like(out["rgb"]); g_alpha = torch.empty_like(out["alpha"]); g_depth = torch.empty_like(out["depth"])
+    g_w = torch.empty_like(out["weights"])
+    sums = torch.empty(16, device=dev, dtype=f32)
+    extra = g_rgb_extra.reshape(-1, 3).contiguous() if g_rgb_extra is not None else None
+    _lib.count(1); check(lib().ia_ngp_loss(C.c_int(n), C.c_int(S), C.c_int(patch_rays), ptr(out["rgb"], f32), ptr(out["alpha"], f32),
+                                           ptr(out["depth"], f32), ptr(out["weights"], f32),
+                                           ptr(target_rgb.reshape(-1, 3).contiguous(), f32), ptr(target_alpha.reshape(-1).contiguous(), f32),
+                                           C.c_float(w_rgb), C.c_float(w_alpha), C.c_float(w_reg), C.c_float(w_depth_reg), ptr(extra, f32),
+                                           ptr(scale_dev), ptr(g_rgb), ptr(g_alpha), ptr(g_depth), ptr(g_w), ptr(sums), stream()))
+    losses = {"mse_loss": sums[4], "loss_alpha_coarse": sums[5], "reg_alpha": sums[6], "reg_density": sums[7],
+              "loss_depth_reg": sums[10], "loss": sums[12]}
+    return losses, g_rgb, g_alpha, g_depth, g_w
+
+
 def pose_grad(scene: Scene, lbs_voxel, xd, best, denc, count, grad_tfs):
     """d loss / d tfs (+=) by implicit differentiation of the Broyden roots (deformer_torch.py:50-67)"""
     _lib.count(1); check(lib().ia_pose_grad(C.byref(scene.c_struct()), ptr(lbs_voxel.reshape(24, -1).contiguous(), f32), ptr(xd, f32),
