@@ -69,7 +69,9 @@ __global__ void threshold_kernel(const float* __restrict__ pooled, int N, int G,
     count[i] = 0;
 }
 
-// find with path halving; parent[x] >= x always holds (roots are the largest index), so the racy shortcut writes are safe
+// find with path halving, for the union pass only.  There parent[x] >= x always holds (roots are the largest index),
+// only roots are CAS-linked, and a halving write stores an ancestor into a non-root entry: a racy write can undo
+// another thread's shortcut but never points a cell outside its tree.
 __device__ __forceinline__ int uf_find(int* parent, int i) {
     for (;;) {
         const int p = parent[i];
@@ -110,10 +112,22 @@ __global__ void union_kernel(int* __restrict__ parent, int G) {
             }
 }
 
+// read-only walk to the root, for the flatten pass.  Each thread of that pass stores its root into its own entry only,
+// so every value a walk reads is an ancestor or the root.  A halving write here could replace a root that a finished
+// thread had stored with a non-root ancestor, and select_pack_kernel would drop that cell.
+__device__ __forceinline__ int uf_root(const int* parent, int i) {
+    for (;;) {
+        const int p = parent[i];
+        if (p == i) return i;
+        i = p;
+    }
+}
+
+// after this pass parent is flat: every on-cell holds its component's label
 __global__ void flatten_count_kernel(int* __restrict__ parent, int* __restrict__ count, int N) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     if (i >= N || parent[i] < 0) return;
-    const int r = uf_find(parent, i);
+    const int r = uf_root(parent, i);
     parent[i] = r;
     atomicAdd(&count[r], 1);
 }
