@@ -169,6 +169,35 @@ int ia_pack_occupancy(const uint8_t* field_bool, uint32_t* bits, int G, ia_strea
 int ia_occupancy_build(const float* density, int G, uint8_t* field_out, uint32_t* bits_out, void* workspace,
                        size_t workspace_bytes, ia_stream_t stream);
 
+/* Marching cubes (replaces skimage.measure.marching_cubes in utils/marching_cubes.py:29-30 and trimesh's
+ * matrix_to_marching_cubes in DensityGrid.export_mesh, density_grid.py:112-116).  field [nx][ny][nz] fp32, x slowest;
+ * nx, ny, nz >= 2 and 3*nx*ny*nz < 2^31, else IA_EINVAL (and the *_bytes queries return 0).  A lattice point is above
+ * iff v > level; every lattice edge with exactly one end above carries one vertex, id ordered by (linear index of the
+ * lower end, axis).  Triangles come from the generated table ia_mc_table.cuh, ordered by (cube linear index, table
+ * order).  Two calls share the caller's workspace of ia_mc_workspace_bytes(nx, ny, nz) bytes:
+ *   ia_mc_count : counts [3] int64 (device) = {n_verts, n_faces, number of non-finite field values}
+ *   ia_mc_emit  : verts [n_verts][3] = (p / div) * ext + origin per component (p: index-space position, the crossing
+ *                 axis at i + (level - v_lo) / (v_hi - v_lo); ext_origin [6] device = ext xyz, origin xyz), faces
+ *                 [n_faces][3] int32; flip = 0: triangle normals point to the above side (object {v < level}),
+ *                 flip != 0: to the other side.  n_verts / n_faces: the counts of ia_mc_count. */
+size_t ia_mc_workspace_bytes(int nx, int ny, int nz);
+int ia_mc_count(const float* field, int nx, int ny, int nz, float level, void* workspace, size_t workspace_bytes,
+                long long* counts, ia_stream_t stream);
+int ia_mc_emit(const float* field, int nx, int ny, int nz, float level, int flip, float div, const float* ext_origin,
+               const void* workspace, size_t workspace_bytes, int n_verts, int n_faces, float* verts, int* faces,
+               ia_stream_t stream);
+
+/* Largest connected component of a triangle mesh (trimesh.Trimesh.split + the max-area choice of
+ * utils/marching_cubes.py:36-45 + submesh): faces sharing a vertex are connected; a component's area is the exact sum
+ * of its faces' float32 0.5 |(b - a) x (c - a)| in 2^-32 fixed point (exact while below 2^32 units^2); the largest area
+ * wins, an exact tie goes to the component holding the lowest face index.  The kept faces keep their order, the kept
+ * vertices their ascending order, re-indexed: verts_out [n_verts][3] and faces_out [n_faces][3] (capacity) receive
+ * kept [2] int64 (device) = {vertices, faces} rows.  workspace >= ia_mc_component_workspace_bytes(n_verts, n_faces). */
+size_t ia_mc_component_workspace_bytes(int n_verts, int n_faces);
+int ia_mc_largest_component(const float* verts, const int* faces, int n_verts, int n_faces, void* workspace,
+                            size_t workspace_bytes, float* verts_out, int* faces_out, long long* kept,
+                            ia_stream_t stream);
+
 /* Fused eval renderer.  Replaces Raymarcher.render_test (renderers/raymarcher_acc.py:82-138) together with
  * raymarch_test / composite_test (renderers/cuda/raymarcher.cpp:16-29,65-75), SNARFDeformer.deform_test
  * (deformers/snarf_deformer.py:126-141), fuse_broyden + filter (fuse_cuda.cpp:14-25, filter.cpp:12-18) and

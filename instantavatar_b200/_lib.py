@@ -28,6 +28,7 @@ SYMBOLS = [
     "ia_tcnn_encoder_backward", "ia_tcnn_mlp_forward", "ia_tcnn_mlp_backward", "ia_render_fwd_peer", "ia_occupancy_query_peer", "ia_peer_reduce_check",
     "ia_peer_flags_to_found", "ia_adam_step_dev_peer", "ia_occupancy_query_ordered", "ia_train_fwd_split", "ia_train_fwd_workspace_bytes",
     "ia_nv_workspace_bytes", "ia_nv_grid_build", "ia_nv_nearest", "ia_nv_pose_grad", "ia_ngp_loss",
+    "ia_mc_workspace_bytes", "ia_mc_count", "ia_mc_emit", "ia_mc_component_workspace_bytes", "ia_mc_largest_component",
 ]
 
 
@@ -74,6 +75,8 @@ def lib():
         _lib.ia_tcnn_backward_scratch_bytes.restype = C.c_size_t
         _lib.ia_train_fwd_workspace_bytes.restype = C.c_size_t
         _lib.ia_nv_workspace_bytes.restype = C.c_size_t
+        _lib.ia_mc_workspace_bytes.restype = C.c_size_t
+        _lib.ia_mc_component_workspace_bytes.restype = C.c_size_t
         for s in SYMBOLS:
             getattr(_lib, s)  # fail loudly on a stale library
         if _lib.ia_abi_version() != 1:

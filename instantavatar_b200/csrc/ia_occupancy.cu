@@ -11,6 +11,7 @@
 #include <stdint.h>
 
 #include "ia_host.h"
+#include "ia_union_find.cuh"
 
 namespace {
 
@@ -69,32 +70,6 @@ __global__ void threshold_kernel(const float* __restrict__ pooled, int N, int G,
     count[i] = 0;
 }
 
-// find with path halving, for the union pass only.  There parent[x] >= x always holds (roots are the largest index),
-// only roots are CAS-linked, and a halving write stores an ancestor into a non-root entry: a racy write can undo
-// another thread's shortcut but never points a cell outside its tree.
-__device__ __forceinline__ int uf_find(int* parent, int i) {
-    for (;;) {
-        const int p = parent[i];
-        if (p == i) return i;
-        const int gp = parent[p];
-        if (gp != p) parent[i] = gp;
-        i = p;
-    }
-}
-
-// roots are the largest linear index of the component (the label the reference's max-flood converges to)
-__device__ __forceinline__ void uf_union(int* parent, int a, int b) {
-    for (;;) {
-        a = uf_find(parent, a);
-        b = uf_find(parent, b);
-        if (a == b) return;
-        if (a < b) { const int t = a; a = b; b = t; }
-        const int old = atomicCAS(&parent[b], b, a);
-        if (old == b) return;
-        b = old;
-    }
-}
-
 __global__ void union_kernel(int* __restrict__ parent, int G) {
     const int i = blockIdx.x * blockDim.x + threadIdx.x;
     const int N = G * G * G;
@@ -110,17 +85,6 @@ __global__ void union_kernel(int* __restrict__ parent, int G) {
                 const int j = (xx * G + yy) * G + zz;
                 if (parent[j] >= 0) uf_union(parent, i, j);
             }
-}
-
-// read-only walk to the root, for the flatten pass.  Each thread of that pass stores its root into its own entry only,
-// so every value a walk reads is an ancestor or the root.  A halving write here could replace a root that a finished
-// thread had stored with a non-root ancestor, and select_pack_kernel would drop that cell.
-__device__ __forceinline__ int uf_root(const int* parent, int i) {
-    for (;;) {
-        const int p = parent[i];
-        if (p == i) return i;
-        i = p;
-    }
 }
 
 // after this pass parent is flat: every on-cell holds its component's label

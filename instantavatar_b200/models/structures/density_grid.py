@@ -136,3 +136,9 @@ class DensityGrid(torch.nn.Module):
             _, d = deformer(coords.reshape(-1, 3), net)
             density = torch.maximum(density, d.reshape(density.shape))
         self.build_from_density(density)
+
+    def export_mesh(self):
+        """density_grid.py:112-116 (trimesh.voxel.ops.matrix_to_marching_cubes(density_field, pitch=1.0)): the boundary of
+        the occupied cells as a closed mesh in voxel-index units, meshed on the GPU (mesh.occupancy_surface)."""
+        from ...mesh import occupancy_surface, to_mesh
+        return to_mesh(*occupancy_surface(self.density_field))

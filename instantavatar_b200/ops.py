@@ -66,6 +66,53 @@ def occupancy_build(density: torch.Tensor, bits=None, want_field=True, workspace
     return field, bits
 
 
+def mc_count(field: torch.Tensor, level: float, workspace=None):
+    """marching cubes, first call: field [nx,ny,nz] fp32 -> (counts int64 [3] = n_verts, n_faces, n_nonfinite (device),
+    workspace holding the classification and scans for mc_emit)"""
+    fp = ptr(field, f32)
+    nx, ny, nz = field.shape
+    nbytes = lib().ia_mc_workspace_bytes(nx, ny, nz)
+    if nbytes == 0:
+        raise RuntimeError(f"libia_b200: marching cubes needs a lattice of at least 2x2x2 with 3*nx*ny*nz < 2^31, got {tuple(field.shape)}")
+    if workspace is None or workspace.numel() < nbytes:
+        workspace = torch.empty(nbytes, device=field.device, dtype=torch.uint8)
+    counts = torch.empty(3, device=field.device, dtype=torch.int64)
+    _lib.count(6); check(lib().ia_mc_count(fp, nx, ny, nz, C.c_float(level), ptr(workspace), C.c_size_t(nbytes),
+                                           ptr(counts, torch.int64), stream()))
+    return counts, workspace
+
+
+def mc_emit(field: torch.Tensor, level: float, workspace, n_verts: int, n_faces: int, flip: bool, div: float,
+            ext_origin: torch.Tensor):
+    """marching cubes, second call (after mc_count on the same field): -> vertices fp32 [V,3] = (p / div) * ext + origin,
+    faces int32 [F,3]; ext_origin fp32 [6] (device) = ext xyz, origin xyz"""
+    nx, ny, nz = field.shape
+    dev = field.device
+    verts = torch.empty((n_verts, 3), device=dev, dtype=f32)
+    faces = torch.empty((n_faces, 3), device=dev, dtype=torch.int32)
+    _lib.count(2); check(lib().ia_mc_emit(ptr(field, f32), nx, ny, nz, C.c_float(level), C.c_int(1 if flip else 0), C.c_float(div),
+                                          ptr(ext_origin, f32), ptr(workspace), C.c_size_t(workspace.numel()), C.c_int(n_verts),
+                                          C.c_int(n_faces), ptr(verts), ptr(faces), stream()))
+    return verts, faces
+
+
+def mc_largest_component(verts: torch.Tensor, faces: torch.Tensor):
+    """largest-area connected component of (verts fp32 [V,3], faces int32 [F,3]), compacted in the original order.
+    Reads the kept counts back (one device synchronisation)."""
+    V, F = verts.shape[0], faces.shape[0]
+    dev = verts.device
+    nbytes = lib().ia_mc_component_workspace_bytes(V, F)
+    if nbytes == 0:
+        raise RuntimeError(f"libia_b200: component extraction needs 0 < V, F < 2^31 - 1, got V={V}, F={F}")
+    workspace = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+    verts_out = torch.empty_like(verts); faces_out = torch.empty_like(faces)
+    kept = torch.empty(2, device=dev, dtype=torch.int64)
+    _lib.count(12); check(lib().ia_mc_largest_component(ptr(verts, f32), ptr(faces, torch.int32), C.c_int(V), C.c_int(F), ptr(workspace),
+                                                       C.c_size_t(nbytes), ptr(verts_out), ptr(faces_out), ptr(kept), stream()))
+    kv, kf = kept.tolist()
+    return verts_out[:kv], faces_out[:kf]
+
+
 def occupancy_batches(G: int, passes: int) -> int:
     """number of scheduling batches of the occupancy query (32 // passes neighbouring cells with all their passes each)"""
     cpb = 32 // passes
