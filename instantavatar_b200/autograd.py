@@ -1,7 +1,7 @@
 """torch.autograd glue for the fused training kernels.
 
 The reference differentiates ~20 ATen ops + two tiny-cuda-nn modules (SURVEY.md §3.2); here one custom Function wraps
-`ia_train_fwd` (forward) and `ia_composite_bwd` + `ia_ngp_backward` (backward): it returns the per-ray outputs the
+`ia_train_fwd_split` (forward) and `ia_composite_bwd` + `ia_ngp_backward` (backward): it returns the per-ray outputs the
 loss consumes (rgb, depth, alpha and the dense per-sample weights) and produces gradients for the two flat parameter
 tensors `encoder.params` / `color_net.params`.  When the bone transforms `tfs` carry an autograd history (pose
 optimisation, DNeRF.py:112-127 with `optimize_SMPL.enable`), `ia_pose_grad` additionally returns d loss / d tfs -- the

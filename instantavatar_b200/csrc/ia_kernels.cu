@@ -13,10 +13,8 @@ using namespace ia;
 static int g_render_rays = 4;  // rays per warp (32 / 16 / 8 / 4), tunable through ia_set_option
 static int g_render_plan = 1;  // longest-first tile scheduling (needs the large workspace)
 static int g_query_warps = 12;   // same for the point-query kernel (12 / 16 / 20; 16 and 20 only without xc output)
-static int g_train_rays = 2;   // rays per warp of the training forward (4 / 2 / 1)
-static int g_query_lanes = 0;  // lanes per point of the list-mode point query (split training forward): 0 = auto, 1 / 2 / 4
+static int g_query_lanes = 0;  // lanes per point of the list-mode point query (training forward): 0 = auto, 1 / 2 / 4
 static int g_occ_lanes = 0;    // lanes per point of the occupancy passes: 0 = 1 (more were measured slower, see occupancy_query_impl)
-int ia_train_rays_per_warp() { return g_train_rays; }
 
 #include "ia_host.h"
 #include "ia_scene.cuh"
@@ -902,11 +900,6 @@ int ia_set_option(const char* name, int value) {
     if (!strcmp(name, "query_lanes_per_sample")) {
         IA_REQUIRE(value == 0 || value == 1 || value == 2 || value == 4);
         g_query_lanes = value;
-        return IA_OK;
-    }
-    if (!strcmp(name, "train_rays_per_warp")) {
-        IA_REQUIRE(value == 4 || value == 2 || value == 1);
-        g_train_rays = value;
         return IA_OK;
     }
     return set_err(IA_EINVAL, "unknown option: %s", name);

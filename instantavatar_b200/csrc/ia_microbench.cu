@@ -1,6 +1,6 @@
 // ia_microbench.cu -- the measured ceiling the roofline of the gather-bound kernels is quoted against (bench.py).
 //
-// deform_query_kernel / render_fwd_kernel / train_fwd_kernel spend their memory time in one access shape: every lane
+// deform_query_kernel / render_fwd_kernel spend their memory time in one access shape: every lane
 // gathers its own trilinear footprint of the skinning-transform field -- 4 x-pair records of 96 bytes = 12 sectors,
 // 24 x LDG.E.128 -- from a 50 MB table, and the next address depends on the loaded data (a Broyden
 // iterate).  This kernel issues exactly that shape and nothing else (no solver arithmetic beyond the 96 FMAs that

@@ -126,11 +126,8 @@ class DNeRFModel(torch.nn.Module):
                                           is_refine=bool(self._pose_cfg.get("is_refine", False)))
 
     def configure_parallel(self, world_size: int):
-        """Ray-sharded training over `world_size` ranks.  With 1/G of the step's rays a rank has fewer ray tiles than resident
-        warps and the forward kernel's time is the critical path of its heaviest tile, so from 4 ranks on the tiles shrink to
-        one ray with 32-deep look-ahead (results do not depend on the tile)."""
+        """Ray-sharded training over `world_size` ranks."""
         self.world_size = int(world_size)
-        ops.set_option("train_rays_per_warp", 1 if self.world_size >= 4 else 2)
         self.optimizer.prepare(self.world_size)
 
     def scheduler_step(self):

@@ -252,21 +252,26 @@ def gather_ceiling(field: torch.Tensor, iters: int = 200, warps: int = 12, coher
 
 
 # the library's tuning knobs (ia_set_option) and their defaults, mirrored here so that a caller can change one temporarily
-_OPTIONS = {"render_rays_per_warp": 4, "render_plan": 1, "render_warps": 12, "query_warps": 12, "train_rays_per_warp": 2,
-            "train_split": 1, "query_lanes_per_sample": 0, "occupancy_lanes_per_point": 0}
+_OPTIONS = {"render_rays_per_warp": 4, "render_plan": 1, "render_warps": 12, "query_warps": 12,
+            "query_lanes_per_sample": 0, "occupancy_lanes_per_point": 0}
+# options of the retired one-kernel training forward, still readable (bench.py reports them) at the only value the
+# three-launch forward has: it is always the forward (train_split) and runs one warp per ray (train_rays_per_warp)
+_FIXED_OPTIONS = {"train_split": 1, "train_rays_per_warp": 1}
 _train_ws: dict = {}
 
 
 def set_option(name: str, value: int):
-    if name == "train_split":   # host-side choice between ia_train_fwd_split (1, default) and the fused ia_train_fwd (0)
-        _OPTIONS[name] = int(bool(value))
+    if name in _FIXED_OPTIONS:
+        if int(value) != _FIXED_OPTIONS[name]:
+            raise ValueError(f"{name} can only be {_FIXED_OPTIONS[name]}: the one-kernel training forward it configured "
+                             "was retired")
         return
     check(lib().ia_set_option(name.encode(), C.c_int(value)))
     _OPTIONS[name] = int(value)
 
 
 def get_option(name: str) -> int:
-    return _OPTIONS[name]
+    return _FIXED_OPTIONS[name] if name in _FIXED_OPTIONS else _OPTIONS[name]
 
 
 def new_stats(device) -> torch.Tensor:
@@ -344,8 +349,9 @@ def ngp_forward(scene: Scene, x):
 # ------------------------------------------------------------------------------------------------------------------
 # training path
 # ------------------------------------------------------------------------------------------------------------------
-def train_fwd(scene: Scene, rays_o, rays_d, near, far, bg=None, jitter=None, noise=None, stats=None, workspace=None):
-    """Fused Raymarcher.render_train (raymarcher_acc.py:140-186).  Returns (outputs, saved-for-backward)."""
+def train_fwd(scene: Scene, rays_o, rays_d, near, far, bg=None, jitter=None, noise=None, stats=None):
+    """Fused Raymarcher.render_train (raymarcher_acc.py:140-186) in three launches (march -> sample list -> point query
+    over the list -> compositing).  Returns (outputs, saved-for-backward)."""
     n = rays_o.numel() // 3
     dev = rays_o.device
     S = _lib.IA_MAX_SAMPLES
@@ -355,24 +361,14 @@ def train_fwd(scene: Scene, rays_o, rays_d, near, far, bg=None, jitter=None, noi
              "xc": torch.empty((n, S, 3), device=dev, dtype=f32), "z": torch.empty((n, S), device=dev, dtype=f32),
              "count": torch.empty(n, device=dev, dtype=torch.int32), "best": torch.empty((n, S), device=dev, dtype=torch.int8)}
     s = scene.c_struct()
-    if _OPTIONS["train_split"]:
-        # three launches (march -> sample list -> point query over the list -> compositing), same results: every 32-sample
-        # batch of the step is an independent work item instead of a tile's samples being walked inside one warp
-        key = (dev, n)
-        ws = _train_ws.get(key)
-        if ws is None:   # kept for the life of the process: a captured CUDA graph may reference it
-            ws = _train_ws[key] = torch.empty(64 + n * S, device=dev, dtype=torch.int32)
-        _lib.count(3); check(lib().ia_train_fwd_split(C.byref(s), ptr(rays_o, f32), ptr(rays_d, f32), ptr(near, f32), ptr(far, f32), C.c_int(n),
-                                                      ptr(bg), ptr(jitter), ptr(noise), ptr(out["rgb"]), ptr(out["depth"]), ptr(out["alpha"]),
-                                                      ptr(out["weights"]), ptr(saved["sigma"]), ptr(saved["rgb"]), ptr(saved["xc"]), ptr(saved["z"]),
-                                                      ptr(saved["count"]), ptr(saved["best"]), ptr(ws), C.c_size_t(ws.numel() * 4), ptr(stats), stream()))
-        return out, saved
-    if workspace is None:
-        workspace = torch.empty(64, device=dev, dtype=torch.int32)
-    _lib.count(1); check(lib().ia_train_fwd(C.byref(s), ptr(rays_o, f32), ptr(rays_d, f32), ptr(near, f32), ptr(far, f32), C.c_int(n),
-                                            ptr(bg), ptr(jitter), ptr(noise), ptr(out["rgb"]), ptr(out["depth"]), ptr(out["alpha"]),
-                                            ptr(out["weights"]), ptr(saved["sigma"]), ptr(saved["rgb"]), ptr(saved["xc"]), ptr(saved["z"]),
-                                            ptr(saved["count"]), ptr(saved["best"]), ptr(workspace), ptr(stats), stream()))
+    key = (dev, n)
+    ws = _train_ws.get(key)
+    if ws is None:   # kept for the life of the process: a captured CUDA graph may reference it
+        ws = _train_ws[key] = torch.empty(64 + n * S, device=dev, dtype=torch.int32)
+    _lib.count(3); check(lib().ia_train_fwd_split(C.byref(s), ptr(rays_o, f32), ptr(rays_d, f32), ptr(near, f32), ptr(far, f32), C.c_int(n),
+                                                  ptr(bg), ptr(jitter), ptr(noise), ptr(out["rgb"]), ptr(out["depth"]), ptr(out["alpha"]),
+                                                  ptr(out["weights"]), ptr(saved["sigma"]), ptr(saved["rgb"]), ptr(saved["xc"]), ptr(saved["z"]),
+                                                  ptr(saved["count"]), ptr(saved["best"]), ptr(ws), C.c_size_t(ws.numel() * 4), ptr(stats), stream()))
     return out, saved
 
 

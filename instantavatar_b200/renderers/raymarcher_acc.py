@@ -3,9 +3,9 @@
 Same constructor, `initialize(N)`, `__call__(rays, model, eval_mode, noise, bg_color)` and result dictionary as the
 reference.  When `model` is bound to a SNARFDeformer + NeRFNGPNet pair (a `BoundModel`, or the reference's
 `lambda x, _: self.deformer(x, self.net_coarse, eval_mode)` closure) the whole per-ray path -- occupancy-grid march,
-Broyden root finding, hash grid + MLPs, compositing -- runs as one fused kernel (`ia_render_fwd`, and the
-`ia_train_fwd/bwd` pair for training) instead of the reference's host-synchronous window loop.  An SMPLDeformer (one
-frame) + NeRFNGPNet pair runs the same kernels with the nearest-vertex deform stage.
+Broyden root finding, hash grid + MLPs, compositing -- runs as one fused kernel (`ia_render_fwd`; for training
+`ia_train_fwd_split` with `ia_composite_bwd` + `ia_ngp_backward`) instead of the reference's host-synchronous window
+loop.  An SMPLDeformer (one frame) + NeRFNGPNet pair runs the same kernels with the nearest-vertex deform stage.
 """
 from __future__ import annotations
 

@@ -84,6 +84,23 @@ def upload(sc, device="cuda"):
     return scene, {"voxel_d": vd, "aabb": aabb}
 
 
+def patch_rays(sc, seed=0):
+    """two 16x16 pixel patches on the body of the 512x512 demo camera, with seeded jitter, noise and background:
+    (o, d, near, far, jitter, noise, bg)"""
+    fr = sc["frame"]
+    o, d, near, far = oscene.camera_rays(fr, 512, 512)
+    idx = []
+    for (y0, x0) in ((200, 240), (300, 250)):
+        ys, xs = np.arange(y0, y0 + 16), np.arange(x0, x0 + 16)
+        idx.append((ys[:, None] * 512 + xs[None]).ravel())
+    idx = np.concatenate(idx)
+    rng = np.random.default_rng(seed)
+    jitter = rng.random((len(idx), 256), dtype=np.float32)
+    noise = rng.normal(0, 1, (len(idx), 256)).astype(np.float32)
+    bg = rng.random((len(idx), 3), dtype=np.float32)
+    return o[idx], d[idx], near[idx], far[idx], jitter, noise, bg
+
+
 def oracle_model(sc, eval_mode=True):
     return lambda p: orender.deform_query(p, sc["frame"], sc["subj"], sc["net"], eval_mode)
 

@@ -6,6 +6,7 @@ import pytest
 from oracle import render as orender
 from oracle import scene as oscene
 from oracle import testing as scene_util
+from oracle import train_fwd_golden
 
 pytestmark = pytest.mark.gpu
 
@@ -154,66 +155,29 @@ def test_invalid_arguments_are_reported(sc, dev):
         ops.render_fwd(scene, o.double(), o, n, n)
 
 
-def _train_both(scene, o, d, near, far, bg, jitter, noise):
-    """(split forward, fused forward) outputs + saved state on the same inputs"""
-    import torch
-    from instantavatar_b200 import ops
-    res = []
-    try:
-        for split in (1, 0):
-            ops.set_option("train_split", split)
-            stats = ops.new_stats("cuda")
-            out, saved = ops.train_fwd(scene, _t(o), _t(d), _t(near), _t(far), _t(bg), _t(jitter) if jitter is not None else None,
-                                       _t(noise) if noise is not None else None, stats)
-            torch.cuda.synchronize()
-            res.append((out, saved, ops.stats_dict(stats)))
-    finally:
-        ops.set_option("train_split", 1)
-    return res
-
-
-def _assert_train_equal(a, b):
-    import torch
-    (out0, saved0, st0), (out1, saved1, st1) = a, b
-    assert st0["samples"] == st1["samples"] and st0["net_evals"] == st1["net_evals"]
-    for k in out0:
-        assert torch.equal(out0[k], out1[k]), k
-    assert torch.equal(saved0["count"], saved1["count"]) and torch.equal(saved0["best"], saved1["best"])
-    live = torch.arange(saved0["sigma"].shape[1], device="cuda")[None] < saved0["count"].long()[:, None]
-    for k in ("sigma", "z", "rgb", "xc"):
-        assert torch.equal(saved0[k][live], saved1[k][live]), k
+def _train(sc, scene, case):
+    """one training forward on a case of the golden, checked against it -> (inputs, outputs, saved state, stats)"""
+    inp = train_fwd_golden.inputs(sc, case)
+    out, saved, st = train_fwd_golden.run(scene, inp)
+    train_fwd_golden.assert_matches(case, out, saved, st)
+    return inp, out, saved, st
 
 
 def test_training_forward_edge_cases(sc, dev):
-    """training forward (split and fused forms, which must agree bit for bit): empty occupancy -> background and an empty
-    sample list; full occupancy -> 256 samples on every ray (list at capacity); ragged ray counts; no jitter / noise"""
-    import dataclasses
-    import torch
-    from instantavatar_b200 import ops
+    """training forward, every case equal to its golden (the retired one-kernel form's result): empty occupancy ->
+    background and an empty sample list; full occupancy -> 256 samples on every ray (list at capacity); ragged ray
+    counts; no jitter / noise"""
     scene, _ = dev
-    rng = np.random.default_rng(11)
-    idx = (np.arange(250, 258)[:, None] * 512 + np.arange(244, 260)[None]).ravel()   # 128 rays on the body
-    o, d, near, far = _rays(sc, idx)
-    n = len(idx)
-    bg = rng.random((n, 3)).astype(np.float32)
-    jitter = rng.random((n, 256)).astype(np.float32)
-    noise = rng.normal(0, 1, (n, 256)).astype(np.float32)
     # --- empty occupancy ---
-    empty = dataclasses.replace(scene, occ_bits=ops.pack_occupancy(torch.zeros((64, 64, 64), dtype=torch.bool, device="cuda")))
-    a, b = _train_both(empty, o, d, near, far, bg, jitter, noise)
-    _assert_train_equal(a, b)
-    out, saved, st = a
-    np.testing.assert_array_equal(out["rgb"].cpu().numpy(), bg)
+    inp, out, saved, st = _train(sc, scene, "empty")
+    np.testing.assert_array_equal(out["rgb"].cpu().numpy(), inp["bg"])
     assert st["samples"] == 0 and not out["alpha"].any() and not out["weights"].any() and not saved["count"].any()
     assert (saved["best"] == -1).all()
     # --- full occupancy: every step of every ray is a sample ---
-    full = dataclasses.replace(scene, occ_bits=ops.pack_occupancy(torch.ones((64, 64, 64), dtype=torch.bool, device="cuda")))
-    a, b = _train_both(full, o, d, near, far, bg, jitter, noise)
-    _assert_train_equal(a, b)
-    assert (a[1]["count"] >= 255).all() and a[2]["samples"] == int(a[1]["count"].sum())   # (near + 256 dt may round to far)
-    assert float(a[0]["alpha"].max()) > 0.5
+    inp, out, saved, st = _train(sc, scene, "full")
+    assert (saved["count"] >= 255).all() and st["samples"] == int(saved["count"].sum())   # (near + 256 dt may round to far)
+    assert float(out["alpha"].max()) > 0.5
     # --- ragged sizes (partial warps / blocks), without jitter and noise ---
     for m in (1, 7, 33, 127):
-        a, b = _train_both(scene, o[:m], d[:m], near[:m], far[:m], bg[:m], None, None)
-        _assert_train_equal(a, b)
-        assert a[0]["rgb"].shape == (m, 3)
+        inp, out, saved, st = _train(sc, scene, f"ragged_{m}")
+        assert out["rgb"].shape == (m, 3)

@@ -4,9 +4,9 @@ import numpy as np
 import pytest
 
 from oracle import render as orender
-from oracle import scene as oscene
 from oracle import testing as scene_util
 from oracle import torch_ref
+from oracle import train_fwd_golden
 
 pytestmark = pytest.mark.gpu
 
@@ -22,22 +22,6 @@ def dev(sc):
     scene, extra = scene_util.upload(sc)
     torch.cuda.synchronize()
     return scene, extra
-
-
-def patch_rays(sc, seed=0):
-    """two 16x16 pixel patches on the body of the 512x512 demo camera"""
-    fr = sc["frame"]
-    o, d, near, far = oscene.camera_rays(fr, 512, 512)
-    idx = []
-    for (y0, x0) in ((200, 240), (300, 250)):
-        ys, xs = np.arange(y0, y0 + 16), np.arange(x0, x0 + 16)
-        idx.append((ys[:, None] * 512 + xs[None]).ravel())
-    idx = np.concatenate(idx)
-    rng = np.random.default_rng(seed)
-    jitter = rng.random((len(idx), 256), dtype=np.float32)
-    noise = rng.normal(0, 1, (len(idx), 256)).astype(np.float32)
-    bg = rng.random((len(idx), 3), dtype=np.float32)
-    return o[idx], d[idx], near[idx], far[idx], jitter, noise, bg
 
 
 def rel_err(a, b):
@@ -88,7 +72,7 @@ def test_train_fwd_matches_oracle(sc, dev):
     import torch
     from instantavatar_b200 import ops
     scene, _ = dev
-    rays = patch_rays(sc)
+    rays = scene_util.patch_rays(sc)
     ref = _oracle_train(sc, rays)
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()
     o, d, near, far, jitter, noise, bg = rays
@@ -111,41 +95,44 @@ def test_train_fwd_matches_oracle(sc, dev):
     assert (ref["alpha"] > 0.5).sum() > 100
 
 
-def test_train_fwd_split_equals_fused_bit_for_bit(sc, dev):
-    """ia_train_fwd_split (march -> sample list -> point query -> compositing; the default) and the one-kernel ia_train_fwd
-    must agree in every output and every saved-for-backward value, for every tile shape of the fused kernel"""
+def test_train_fwd_matches_golden_bit_for_bit(sc, dev):
+    """The training forward at every lanes-per-sample setting of its point query equals the others and the stored
+    result of the retired one-kernel form (oracle/train_fwd_golden.py) in every output, every live saved-for-backward
+    value and its stats; and every live sample equals the point query at the posed point the march placed it at"""
     import torch
     from instantavatar_b200 import ops
     scene, _ = dev
-    rays = patch_rays(sc, seed=4)
-    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()
-    o, d, near, far, jitter, noise, bg = rays
+    inp = train_fwd_golden.inputs(sc, "patch")
     res = {}
     try:
-        for name, split, trpw, k in (("split", 1, 2, 1), ("split_k2", 1, 2, 2), ("split_k4", 1, 2, 4), ("split_auto", 1, 2, 0),
-                                     ("fused2", 0, 2, 0), ("fused1", 0, 1, 0)):
-            ops.set_option("train_split", split); ops.set_option("train_rays_per_warp", trpw)
-            ops.set_option("query_lanes_per_sample", k)   # lanes sharing a sample's 13 root finds in the split form's query
-            stats = ops.new_stats("cuda")
-            out, saved = ops.train_fwd(scene, t(o), t(d), t(near), t(far), t(bg), t(jitter), t(noise), stats)
-            torch.cuda.synchronize()
-            res[name] = (out, saved, ops.stats_dict(stats))
+        for k in (1, 2, 4, 0):
+            ops.set_option("query_lanes_per_sample", k)   # lanes sharing a sample's 13 root finds
+            res[k] = train_fwd_golden.run(scene, inp)
     finally:
-        ops.set_option("train_split", 1); ops.set_option("train_rays_per_warp", 2); ops.set_option("query_lanes_per_sample", 0)
-    out0, saved0, st0 = res["split"]
+        ops.set_option("query_lanes_per_sample", 0)
+    out0, saved0, st0 = res[1]
     assert st0["samples"] > 1000
     cnt = saved0["count"].long()
     live = torch.arange(saved0["sigma"].shape[1], device="cuda")[None] < cnt[:, None]   # slots the forward filled
-    for name in ("split_k2", "split_k4", "split_auto", "fused2", "fused1"):
-        out1, saved1, st1 = res[name]
+    for k in (2, 4, 0):
+        out1, saved1, st1 = res[k]
         assert st1["samples"] == st0["samples"] and st1["net_evals"] == st0["net_evals"] and st1["field_loads"] == st0["field_loads"]
-        for k in out0:
-            assert torch.equal(out0[k], out1[k]), (name, k)
+        for name in out0:
+            assert torch.equal(out0[name], out1[name]), (k, name)
         assert torch.equal(saved0["count"], saved1["count"]) and torch.equal(saved0["best"], saved1["best"])
-        for k in ("sigma", "z"):
-            assert torch.equal(saved0[k][live], saved1[k][live]), (name, k)
-        for k in ("rgb", "xc"):
-            assert torch.equal(saved0[k][live], saved1[k][live]), (name, k)
+        for name in ("sigma", "z", "rgb", "xc"):
+            assert torch.equal(saved0[name][live], saved1[name][live]), (k, name)
+    for k, r in res.items():
+        train_fwd_golden.assert_matches("patch", *r)
+    # the point query (point mode of the same kernel instantiation) at each live slot's posed point z * d + o, a
+    # separate multiply and add as the march computes it
+    ray = live.nonzero()[:, 0]
+    t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()
+    pts = saved0["z"][live][:, None] * t(inp["d"])[ray] + t(inp["o"])[ray]
+    rgb, sigma, xc, best = ops.deform_query(scene, pts, eval_mode=False, want_xc=True)
+    torch.cuda.synchronize()
+    for name, v in (("rgb", rgb), ("sigma", sigma), ("xc", xc), ("best", best)):
+        assert torch.equal(v, saved0[name][live]), name
 
 
 def _final_trans_f64(sigma, step):
@@ -171,7 +158,7 @@ def _check_train_backward(sc, dev, case, offset, depth_loss):
     from instantavatar_b200 import ops
     scene, _ = dev
     net = sc["net"]
-    rays = patch_rays(sc, seed=1)
+    rays = scene_util.patch_rays(sc, seed=1)
     o, d, near, far, jitter, noise, bg = rays
     noise = (noise + np.float32(offset)).astype(np.float32)
     rays = (o, d, near, far, jitter, noise, bg)

@@ -18,15 +18,32 @@ def test_shard_layout_covers_and_aligns():
 
 
 def test_option_mirror_defaults_match_the_library_defaults():
+    import ctypes
     import re
     import os
-    from instantavatar_b200 import ops
+    import pytest
+    from instantavatar_b200 import _lib, ops
     src = open(os.path.join(os.path.dirname(ops.__file__), "csrc", "ia_kernels.cu")).read()
     for name, var in (("render_rays_per_warp", "g_render_rays"), ("render_plan", "g_render_plan"), ("query_warps", "g_query_warps"),
-                      ("train_rays_per_warp", "g_train_rays"), ("query_lanes_per_sample", "g_query_lanes"),
-                      ("occupancy_lanes_per_point", "g_occ_lanes")):
+                      ("query_lanes_per_sample", "g_query_lanes"), ("occupancy_lanes_per_point", "g_occ_lanes")):
         m = re.search(r"static int %s = (\d+);" % var, src)
         assert m and int(m.group(1)) == ops._OPTIONS[name], name
+    # the retired one-kernel training forward's options: readable and settable at their one value, never the library's
+    for name in ("train_split", "train_rays_per_warp"):
+        assert ops.get_option(name) == 1
+        ops.set_option(name, 1)
+        for value in (0, 2, 4):
+            with pytest.raises(ValueError, match="retired"):
+                ops.set_option(name, value)
+        assert ops.get_option(name) == 1
+    assert _lib.lib().ia_set_option(b"train_rays_per_warp", ctypes.c_int(1)) == -1
+    assert b"unknown option" in _lib.lib().ia_last_error()
+    # every option bench.py reports is readable
+    bench = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "bench.py")).read()
+    names = set(re.findall(r"""get_option\(\s*["'](\w+)["']""", bench))
+    assert {"train_split", "train_rays_per_warp", "render_rays_per_warp"} <= names, names
+    for name in names:
+        ops.get_option(name)
 
 
 def test_version2_deformer_refuses_training_but_not_construction():

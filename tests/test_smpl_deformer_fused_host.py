@@ -41,8 +41,6 @@ def test_entry_points_without_a_nearest_vertex_form_return_einval():
     s.nv = C.pointer(nv)
     p = C.c_void_p(4096)
     calls = {
-        "ia_train_fwd": lambda: lib.ia_train_fwd(C.byref(s), p, p, p, p, C.c_int(1), None, None, None, p, p, p, p, p, p, p, p, p,
-                                                 p, p, None, None),
         "ia_pose_grad": lambda: lib.ia_pose_grad(C.byref(s), p, p, p, p, p, C.c_int(1), p, None),
         "ia_broyden": lambda: lib.ia_broyden(C.byref(s), p, C.c_int(1), p, p, None, None),
         "ia_render_fwd_peer": lambda: lib.ia_render_fwd_peer(C.byref(s), p, p, p, p, C.c_int(1), None, C.c_int(0), p, p, p, p, p,
