@@ -364,6 +364,17 @@ int ia_ngp_input_grad(const IaScene* scene /*[host]*/, const float* x, const flo
 int ia_pose_grad(const IaScene* scene /*[host]*/, const float* lbs_voxel, const float* xd, const int8_t* best,
                  const float* denc, const int* count, int capacity, float* grad_tfs, ia_stream_t stream);
 
+/* Forward linear-blend skinning of points into n_frames poses in one launch (ForwardDeformer.forward_skinning /
+ * query_weights / skinning_mask, deformers/fast_snarf/deformer_torch.py:118-128,190-218).  Each point's 24 weights are
+ * sampled once from lbs_voxel [24][D][H][W] (ForwardDeformer.lbs_voxel_final; trilinear, align_corners, border padding) at
+ * scale_k * (x_c + offset_k) (offset_k, scale_k [3] as in IaScene), in the summation order of ia_pose_grad; then per frame
+ * T = sum_j w_j tfs[f][j] and x_d = T[:3,:4] [x_c, 1] (DESIGN.md §3, "Forward skinning").  tfs [n_frames][24][4][4],
+ * xc [n][3] -> xd [n_frames][n][3], weights [n][24] (nullable).  n = 0: nothing is done; n_frames < 1, n < 0 or
+ * D / H / W < 1: IA_EINVAL. */
+int ia_skin_points(const float* lbs_voxel, int D, int H, int W, const float* offset_k, const float* scale_k,
+                   const float* tfs, int n_frames, const float* xc, int n, float* xd, float* weights /*nullable*/,
+                   ia_stream_t stream);
+
 /* Pose gradient of the nearest-vertex deformer (scene->nv set).  For each of the first min(*count, capacity) list samples
  * of ia_composite_bwd with best >= 0: l_rz [capacity][3] holds (ray index, z, 0) -- what ia_composite_bwd writes into l_xd
  * when it is given the rays rays_o[i] = (i, 0, 0), rays_d[i] = (0, 1, 0) (z * 0 + i and z * 1 + 0 are exact).  The posed

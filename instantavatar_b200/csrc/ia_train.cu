@@ -1057,6 +1057,32 @@ __device__ __forceinline__ void hash_input_grad(const HashLevels& hl, const __ha
     for (int d = 0; d < 3; d++) g[d] = inside[d] ? g[d] / scale[d] : 0.f;
 }
 
+// Skinning weights of one point (deformer_torch.py:190-201 query_weights: grid_sample of lbs_voxel [24][D][H][W],
+// trilinear, align_corners, BORDER padding) at the sample coordinate q = scale_k * (x + offset_k), x fastest (q[0] spans
+// W).  wts[j] += sum over the 8 corners k = 0..7 (bit 0: x, bit 1: y, bit 2: z) of w_k * lbs_voxel[j][corner k], corners in
+// that order; the caller zeroes wts.  DESIGN.md §3 "Forward skinning"; oracle/skinning_ref.py restates it.
+__device__ __forceinline__ void sample_lbs_weights(const float* __restrict__ lbs_voxel, int D, int H, int W, long V,
+                                                   const float q[3], float wts[24]) {
+    const int dims[3] = {W, H, D};
+    int i0[3], i1[3]; float t1[3];
+#pragma unroll
+    for (int d = 0; d < 3; d++) {
+        float u = ((q[d] + 1.f) / 2.f) * (float)(dims[d] - 1);
+        u = fminf(fmaxf(u, 0.f), (float)(dims[d] - 1));
+        const float fl = floorf(u);
+        i0[d] = (int)fl; i1[d] = min(i0[d] + 1, dims[d] - 1);
+        t1[d] = u - fl;
+    }
+#pragma unroll
+    for (int k = 0; k < 8; k++) {
+        const int ix = (k & 1) ? i1[0] : i0[0], iy = (k & 2) ? i1[1] : i0[1], iz = (k & 4) ? i1[2] : i0[2];
+        const float wk = ((k & 1) ? t1[0] : 1.f - t1[0]) * ((k & 2) ? t1[1] : 1.f - t1[1]) * ((k & 4) ? t1[2] : 1.f - t1[2]);
+        const long off = ((long)iz * H + iy) * W + ix;
+#pragma unroll
+        for (int j = 0; j < 24; j++) wts[j] += wk * __ldg(lbs_voxel + (long)j * V + off);
+    }
+}
+
 struct PoseGradArgs {
     SceneDev sd;
     const float* lbs_voxel;   // [24][D][H][W] (reference layout)
@@ -1097,26 +1123,8 @@ __global__ void __launch_bounds__(256) pose_grad_kernel(const __grid_constant__ 
                 v[1] = -(Ji[1] * g[0] + Ji[4] * g[1] + Ji[7] * g[2]);
                 v[2] = -(Ji[2] * g[0] + Ji[5] * g[1] + Ji[8] * g[2]);
                 xh[0] = x[0]; xh[1] = x[1]; xh[2] = x[2];
-                // ---- skinning weights: trilinear, align_corners, BORDER padding (deformer_torch.py:194-198) ----
                 const float q[3] = {fc.bp.scl[0] * (x[0] + fc.bp.off[0]), fc.bp.scl[1] * (x[1] + fc.bp.off[1]), fc.bp.scl[2] * (x[2] + fc.bp.off[2])};
-                const int dims[3] = {f.W, f.H, f.D};
-                int i0[3], i1[3]; float t1[3];
-#pragma unroll
-                for (int d = 0; d < 3; d++) {
-                    float u = ((q[d] + 1.f) / 2.f) * (float)(dims[d] - 1);
-                    u = fminf(fmaxf(u, 0.f), (float)(dims[d] - 1));
-                    const float fl = floorf(u);
-                    i0[d] = (int)fl; i1[d] = min(i0[d] + 1, dims[d] - 1);
-                    t1[d] = u - fl;
-                }
-#pragma unroll
-                for (int k = 0; k < 8; k++) {
-                    const int ix = (k & 1) ? i1[0] : i0[0], iy = (k & 2) ? i1[1] : i0[1], iz = (k & 4) ? i1[2] : i0[2];
-                    const float wk = ((k & 1) ? t1[0] : 1.f - t1[0]) * ((k & 2) ? t1[1] : 1.f - t1[1]) * ((k & 4) ? t1[2] : 1.f - t1[2]);
-                    const long off = ((long)iz * f.H + iy) * f.W + ix;
-#pragma unroll
-                    for (int j = 0; j < 24; j++) wts[j] += wk * __ldg(a.lbs_voxel + (long)j * V + off);
-                }
+                sample_lbs_weights(a.lbs_voxel, f.D, f.H, f.W, V, q, wts);
             }
         }
         // ---- warp reduction of w_j * v_r * xh_c into the CTA accumulator ----
@@ -1240,6 +1248,81 @@ extern "C" int ia_pose_grad(const IaScene* scene, const float* lbs_voxel, const 
     if (sms <= 0) return set_err(IA_ECUDA, "no CUDA device%s");
     const int n_batches = (capacity + 31) / 32;
     pose_grad_kernel<<<min(sms * 2, (n_batches + 7) / 8), 256, 0, (cudaStream_t)stream>>>(a);
+    IA_CHECK_CUDA(cudaPeekAtLastError());
+    return IA_OK;
+}
+
+namespace {
+constexpr int kSkinFramesPerCta = 8;
+
+struct SkinArgs {
+    const float* lbs_voxel; int D, H, W;
+    const float* offset_k; const float* scale_k;
+    const float* tfs; int n_frames;
+    const float* xc; int n;
+    float* xd; float* weights;
+};
+
+// Forward linear-blend skinning (deformer_torch.py:118-128 forward_skinning, :204-218 skinning_mask): CTA row blockIdx.y
+// serves frames [8 y, 8 y + 8), with their bone transforms' top three rows in shared memory; every point samples its
+// weights once per row and, per frame, forms T = sum_j w_j tfs_j (bones j = 0..23 ascending per entry) and
+// x_d[r] = T[r][0] x + T[r][1] y + T[r][2] z + T[r][3] (columns c = 0..3, left to right).
+__global__ void __launch_bounds__(256) skin_points_kernel(const __grid_constant__ SkinArgs a) {
+    __shared__ float s_tfs[kSkinFramesPerCta][24 * 12];
+    const int f0 = blockIdx.y * kSkinFramesPerCta;
+    const int nf = min(kSkinFramesPerCta, a.n_frames - f0);
+    for (int i = threadIdx.x; i < nf * 24 * 12; i += blockDim.x) {
+        const int fr = i / (24 * 12), r = i % (24 * 12);
+        s_tfs[fr][r] = a.tfs[((long)(f0 + fr) * 24 + r / 12) * 16 + r % 12];
+    }
+    __syncthreads();
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= a.n) return;
+    const float x[3] = {a.xc[(long)p * 3], a.xc[(long)p * 3 + 1], a.xc[(long)p * 3 + 2]};
+    const float q[3] = {a.scale_k[0] * (x[0] + a.offset_k[0]), a.scale_k[1] * (x[1] + a.offset_k[1]), a.scale_k[2] * (x[2] + a.offset_k[2])};
+    float wts[24];
+#pragma unroll
+    for (int j = 0; j < 24; j++) wts[j] = 0.f;
+    sample_lbs_weights(a.lbs_voxel, a.D, a.H, a.W, (long)a.D * a.H * a.W, q, wts);
+    if (a.weights && blockIdx.y == 0) {
+#pragma unroll
+        for (int j = 0; j < 24; j++) a.weights[(long)p * 24 + j] = wts[j];
+    }
+    for (int fr = 0; fr < nf; fr++) {
+        float T[12];
+#pragma unroll
+        for (int e = 0; e < 12; e++) T[e] = 0.f;
+#pragma unroll
+        for (int j = 0; j < 24; j++) {
+#pragma unroll
+            for (int e = 0; e < 12; e++) T[e] += wts[j] * s_tfs[fr][j * 12 + e];
+        }
+        float* out = a.xd + ((long)(f0 + fr) * a.n + p) * 3;
+#pragma unroll
+        for (int r = 0; r < 3; r++) {
+            float v = 0.f;
+            v += T[r * 4] * x[0];
+            v += T[r * 4 + 1] * x[1];
+            v += T[r * 4 + 2] * x[2];
+            v += T[r * 4 + 3];
+            out[r] = v;
+        }
+    }
+}
+}  // namespace
+
+extern "C" int ia_skin_points(const float* lbs_voxel, int D, int H, int W, const float* offset_k, const float* scale_k,
+                              const float* tfs, int n_frames, const float* xc, int n, float* xd, float* weights,
+                              ia_stream_t stream) {
+    IA_REQUIRE(D > 0 && H > 0 && W > 0 && n >= 0);
+    IA_REQUIRE(n_frames > 0 && n_frames <= 65535 * kSkinFramesPerCta);
+    if (n == 0) return IA_OK;
+    IA_REQUIRE(lbs_voxel && offset_k && scale_k && tfs && xc && xd);
+    SkinArgs a;
+    a.lbs_voxel = lbs_voxel; a.D = D; a.H = H; a.W = W; a.offset_k = offset_k; a.scale_k = scale_k;
+    a.tfs = tfs; a.n_frames = n_frames; a.xc = xc; a.n = n; a.xd = xd; a.weights = weights;
+    const dim3 grid((unsigned)((n + 255) / 256), (unsigned)((n_frames + kSkinFramesPerCta - 1) / kSkinFramesPerCta));
+    skin_points_kernel<<<grid, 256, 0, (cudaStream_t)stream>>>(a);
     IA_CHECK_CUDA(cudaPeekAtLastError());
     return IA_OK;
 }

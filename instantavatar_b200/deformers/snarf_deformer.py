@@ -133,6 +133,37 @@ class ForwardDeformer(torch.nn.Module):
         self.field, vd, self.aabb = ops.precompute(self.lbs_voxel_final, tfs, self.offset_kernel, self.scale_kernel)
         self.voxel_d = vd[None]
 
+    @staticmethod
+    def _refuse_grad(*ts):
+        if torch.is_grad_enabled() and any(torch.is_tensor(t) and t.requires_grad for t in ts):
+            raise NotImplementedError("ForwardDeformer.query_weights / forward_skinning are not differentiable here: "
+                                      "detach the inputs or call them under torch.no_grad()")
+
+    def _skin(self, xc, tfs, want_weights):
+        dev = self.lbs_voxel_final.device
+        return ops.skin_points(self.lbs_voxel_final, self.offset_kernel, self.scale_kernel,
+                               tfs.to(dev, torch.float32), xc.to(dev, torch.float32), want_weights)
+
+    def query_weights(self, xc, cond=None, mask=None, mode="bilinear"):
+        """deformer_torch.py:190-201: skinning weights [..., 24] of canonical points xc [..., 3] (grid_sample of
+        lbs_voxel_final, trilinear, align_corners, border padding) on ia_skin_points; `cond` and `mask` are accepted and
+        unused, as in the reference"""
+        if mode != "bilinear":
+            raise ValueError(f"query_weights: only mode='bilinear' (trilinear) is implemented, got {mode!r}")
+        self._refuse_grad(xc)
+        eye = torch.eye(4, device=self.lbs_voxel_final.device).expand(24, 4, 4)
+        _, w = self._skin(xc.reshape(-1, 3), eye, True)
+        return w.reshape(*xc.shape[:-1], 24)
+
+    def forward_skinning(self, xc, cond, tfs, mask=None):
+        """deformer_torch.py:118-128 (skinning_mask, :204-218): canonical points xc [B,N,3] of the rows selected by
+        mask [B,N] (all rows when None) -> deformed points [P,3] under the bone transforms tfs [1,24,4,4]"""
+        self._refuse_grad(xc, tfs)
+        if tfs.reshape(-1, 24, 4, 4).shape[0] != 1:
+            raise ValueError("forward_skinning: tfs holds one pose [1,24,4,4] (ops.skin_points skins into many)")
+        pts = xc[mask] if mask is not None else xc.reshape(-1, 3)
+        return self._skin(pts, tfs, False)[0]
+
 
 class SNARFDeformer:
     def __init__(self, model_path=None, gender="neutral", opt=None, smpl_data: dict | None = None) -> None:

@@ -564,6 +564,22 @@ def pose_grad(scene: Scene, lbs_voxel, xd, best, denc, count, grad_tfs):
                                             ptr(best, torch.int8), ptr(denc, f32), ptr(count), C.c_int(xd.shape[0]), ptr(grad_tfs, f32), stream()))
 
 
+def skin_points(lbs_voxel, offset_k, scale_k, tfs, xc, want_weights=False):
+    """forward linear-blend skinning (deformer_torch.py:118-128,190-218) of canonical points into F poses in one launch:
+    lbs_voxel [24,D,H,W] (any leading 1s), offset_k / scale_k [3], tfs [F,24,4,4], xc [n,3] -> xd [F,n,3]
+    (and the sampled weights [n,24] with want_weights)"""
+    D, H, W = lbs_voxel.shape[-3:]
+    tfs = tfs.reshape(-1, 24, 4, 4).contiguous()
+    xc = xc.reshape(-1, 3).contiguous()
+    F, n = tfs.shape[0], xc.shape[0]
+    xd = torch.empty((F, n, 3), device=xc.device, dtype=f32)
+    weights = torch.empty((n, 24), device=xc.device, dtype=f32) if want_weights else None
+    _lib.count(1); check(lib().ia_skin_points(ptr(lbs_voxel.reshape(24, D, H, W).contiguous(), f32), C.c_int(D), C.c_int(H), C.c_int(W),
+                                              ptr(offset_k.reshape(3).contiguous(), f32), ptr(scale_k.reshape(3).contiguous(), f32),
+                                              ptr(tfs, f32), C.c_int(F), ptr(xc, f32), C.c_int(n), ptr(xd), ptr(weights), stream()))
+    return (xd, weights) if want_weights else xd
+
+
 _RAY_SLOT_CODES: dict = {}
 
 
