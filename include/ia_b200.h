@@ -457,6 +457,46 @@ int ia_mlp_to_half_from_half(const void* enc_mlp_h, const void* col_h, void* mlp
  * sum-reduce-scatter EVERY rank's shard fails ia_grad_check_finite and all ranks skip the step together. */
 int ia_grad_poison_shards(float* grads, long shard_elems, int n_shards, const float* found_inf, ia_stream_t stream);
 
+/* Training batches sampled on the device from device-resident frames (datasets/peoplesnapshot.py:99-151, custom.py:97-149,
+ * utils/sampler.py; DESIGN.md §5.7).  Frames: images [F][H][W][3] uint8 (as decoded, cv2's channel order), masks [F][H][W]
+ * fp32, ray tables rays_o / rays_d [H][W][3] (shared by the frames), near_far [F][2].
+ *
+ * ia_frame_index_build (once per frame set) builds, per frame, three bit sets with per-word exclusive prefix counts in a
+ * caller buffer of ia_frame_index_bytes(F, H, W, patch) bytes (0 for invalid sizes):
+ *   mask   {i : mask[i] != 0} over flat pixels i = y*W + x;
+ *   edge   EdgeSampler's band: i such that the flat window [i - k/2, i - k/2 + k - 1] clipped to [0, H*W) holds two different
+ *          values (cv2.erode / cv2.dilate of mask.reshape(-1), an (H*W) x 1 image; horizontal only, wrapping across rows).
+ *          edge_kernel k = 0: empty;
+ *   centre PatchSampler's valid corners (r, c), 0 <= r < H-P, 0 <= c < W-P, as r*(W-P) + c, where m'[r + P/2][c + P/2] > 0;
+ *          m' is the mask, or with dilate = d > 0 its max over rows / columns y - d/2 .. y - d/2 + d - 1 inside the frame.
+ *          patch P = 0: no centre set (P even, P < H, P < W otherwise).
+ * counts [F][3] int64 receives the three set sizes.  edge_kernel <= 1024, dilate <= 256.
+ *
+ * A 32-bit random word selects element (word * count) >> 32 (64-bit product) of a set of size count.
+ *   ia_sample_edge: rays t < num_mask from the mask set, then num_edge from the edge band, then num_rand uniform over the
+ *     H*W pixels; words [n] (n = num_mask + num_edge + num_rand).  words NULL (index may be NULL): ray t is pixel t, the
+ *     full frame (num_mask = num_edge = 0, num_rand = H*W).  `patch` is the P the index was built with.
+ *   ia_sample_patch: num_patch (<= 1024) patches of P x P; words [1 + 2*num_patch].  Mask branch iff words[0] / 2^32 <
+ *     ratio_mask: distinct centres by Floyd's algorithm (for j = C-n .. C-1, t from words[1 + j - (C-n)] over [0, j]; t,
+ *     or j when t was taken, in that order).  Otherwise r from words[1 + p] over [0, H-P) and c from words[1 + n + p] over
+ *     [0, W-P).  Patch p covers rows r .. r+P-1 and columns c .. c+P-1; its rays are p*P*P + dy*P + dx.
+ * Per ray t from pixel i of `frame`: rgb[t] = img * m + (1 - m) * bg[t] with img = u8 / 255 (IEEE division, no
+ * contraction), alpha[t] = m, rays_o/rays_d[t] = the tables at i, bg_color[t] = bg[t] (bg NULL: 1), near/far[t] =
+ * near_far[frame].  A ray drawn from an empty set (or a mask-branch patch with fewer than num_patch centres) gets NaN in
+ * every output. */
+size_t ia_frame_index_bytes(int F, int H, int W, int patch);
+int ia_frame_index_build(const float* masks, int F, int H, int W, int edge_kernel, int patch, int dilate, void* index,
+                         size_t nbytes, int64_t* counts, ia_stream_t stream);
+int ia_sample_edge(const uint8_t* images, const float* masks, const float* rays_o, const float* rays_d, const float* near_far,
+                   int F, int H, int W, const void* index /*nullable with words*/, int patch, int frame, int num_mask,
+                   int num_edge, int num_rand, const uint32_t* words /*nullable*/, const float* bg /*nullable*/, float* rgb,
+                   float* alpha, float* out_rays_o, float* out_rays_d, float* bg_color, float* near, float* far,
+                   ia_stream_t stream);
+int ia_sample_patch(const uint8_t* images, const float* masks, const float* rays_o, const float* rays_d, const float* near_far,
+                    int F, int H, int W, const void* index, int frame, int num_patch, int patch, double ratio_mask,
+                    const uint32_t* words, const float* bg, float* rgb, float* alpha, float* out_rays_o, float* out_rays_d,
+                    float* bg_color, float* near, float* far, ia_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -697,6 +697,64 @@ def tcnn_mlp_backward(mlp_h, in15, dout3, grad_col=None, want_din=False, grad_sc
     return din
 
 
+def frame_index_bytes(F: int, H: int, W: int, patch: int = 0) -> int:
+    nbytes = int(lib().ia_frame_index_bytes(C.c_int(F), C.c_int(H), C.c_int(W), C.c_int(patch)))
+    if nbytes == 0 and F > 0:
+        raise ValueError(f"no frame index for F={F}, H={H}, W={W}, patch={patch}")
+    return nbytes
+
+
+def frame_index_build(masks, edge_kernel: int = 0, patch: int = 0, dilate: int = 0):
+    """the sampler index of a frame set (EdgeSampler's mask set and band, PatchSampler's centre set): masks [F,H,W] fp32 ->
+    (index: uint8 [ia_frame_index_bytes], counts [F,3] int64 = sizes of the mask, edge and centre sets)"""
+    F, H, W = masks.shape
+    index = torch.empty(frame_index_bytes(F, H, W, patch), device=masks.device, dtype=torch.uint8)
+    counts = torch.zeros((F, 3), device=masks.device, dtype=torch.int64)
+    _lib.count(2); check(lib().ia_frame_index_build(ptr(masks.contiguous(), f32), C.c_int(F), C.c_int(H), C.c_int(W),
+                                                    C.c_int(edge_kernel), C.c_int(patch), C.c_int(dilate), ptr(index),
+                                                    C.c_size_t(index.numel()), ptr(counts), stream()))
+    return index, counts
+
+
+def _sample_outputs(n: int, device):
+    o = {k: torch.empty((n, 3), device=device, dtype=f32) for k in ("rgb", "rays_o", "rays_d", "bg_color")}
+    o.update({k: torch.empty((n,), device=device, dtype=f32) for k in ("alpha", "near", "far")})
+    return o
+
+
+def _sample_ptrs(o):
+    return [ptr(o[k]) for k in ("rgb", "alpha", "rays_o", "rays_d", "bg_color", "near", "far")]
+
+
+def _frame_ptrs(frames):
+    F, H, W = frames["masks"].shape
+    return [ptr(frames["images"], torch.uint8), ptr(frames["masks"], f32), ptr(frames["rays_o"], f32), ptr(frames["rays_d"], f32),
+            ptr(frames["near_far"], f32), C.c_int(F), C.c_int(H), C.c_int(W)]
+
+
+def sample_edge(frames: dict, index, patch: int, frame: int, num_mask: int, num_edge: int, num_rand: int, words=None, bg=None):
+    """EdgeSampler.sample + the dataset's compositing (sampler.py:22-45, peoplesnapshot.py:106-118) in one launch.
+    frames: images [F,H,W,3] uint8, masks [F,H,W], rays_o / rays_d [H,W,3], near_far [F,2]; index of frame_index_build
+    (built with `patch`); words [n] int32 (read as uint32), bg [n,3] (None: 1).  words None: ray t is pixel t (full frame).
+    -> dict of rgb, rays_o, rays_d, bg_color [n,3] and alpha, near, far [n]"""
+    n = num_mask + num_edge + num_rand
+    out = _sample_outputs(n, frames["masks"].device)
+    _lib.count(1); check(lib().ia_sample_edge(*_frame_ptrs(frames), ptr(index), C.c_int(patch), C.c_int(frame), C.c_int(num_mask),
+                                              C.c_int(num_edge), C.c_int(num_rand), ptr(words, torch.int32), ptr(bg, f32),
+                                              *_sample_ptrs(out), stream()))
+    return out
+
+
+def sample_patch(frames: dict, index, frame: int, num_patch: int, patch: int, ratio_mask: float, words, bg):
+    """PatchSampler.sample + the dataset's compositing (sampler.py:56-82) in one launch: words [1 + 2*num_patch] int32,
+    bg [num_patch*P*P, 3] -> dict of [num_patch*P*P, ...] outputs (patch-major) as sample_edge"""
+    out = _sample_outputs(num_patch * patch * patch, frames["masks"].device)
+    _lib.count(1); check(lib().ia_sample_patch(*_frame_ptrs(frames), ptr(index), C.c_int(frame), C.c_int(num_patch), C.c_int(patch),
+                                               C.c_double(ratio_mask), ptr(words, torch.int32), ptr(bg, f32), *_sample_ptrs(out),
+                                               stream()))
+    return out
+
+
 # ------------------------------------------------------------------------------------------------------------------
 # device guard: every operator launches on the current stream OF THE DEVICE ITS TENSORS LIVE ON (one process may hold
 # tensors on several GPUs; function attributes and SM counts are cached per device inside the library)
