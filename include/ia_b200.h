@@ -497,6 +497,35 @@ int ia_sample_patch(const uint8_t* images, const float* masks, const float* rays
                     const uint32_t* words, const float* bg, float* rgb, float* alpha, float* out_rays_o, float* out_rays_d,
                     float* bg_color, float* near, float* far, ia_stream_t stream);
 
+/* Test-split evaluation (DNeRF.py:225-239 and eval.py:93-118; DESIGN.md §3, §5.8).
+ *
+ * ia_test_panel: pred, gt [F][H][W][3] fp32 -> panel [F][H][3W][3] uint8, row y of frame f = [q(gt) | q(pred) | JET[e]] in
+ * the inputs' channel order (cv2's BGR, as the frames are stored), the image the reference's test_step writes.
+ *   q(v) = saturate_u8(rint(float32(v * 255))), rint rounding half to even, as cv2.imwrite converts float images; NaN, and
+ *          products at or above 2^31 (+inf included), give 0 (cv2 on x86-64; aarch64 builds of cv2 saturate those to 255).
+ *   e    = trunc(float32(float32(sqrt((d0^2 + d1^2) + d2^2)) / float32(sqrt 3)) * 255) with d = pred - gt, every operation
+ *          in float32 without contraction (numpy 1.x promotion of DNeRF.py:230).  Where numpy's astype(uint8) is undefined
+ *          the index saturates: e >= 256 -> 255, NaN -> 0.
+ *   JET  = OpenCV's COLORMAP_JET (instantavatar_b200/csrc/ia_jet_lut.cuh).
+ * F * H * W < 2^31.
+ *
+ * ia_image_metrics: per frame f of two uint8 stacks a, b [F][H][W][3] (pixel bytes contiguous; byte strides per frame and per
+ * row, so the pred and gt thirds of a panel are read in place):
+ *   sse[f]     = sum over the 3*H*W bytes of (a - b)^2, exact;
+ *   ssim_fx[f] = sum over the 3 channels and the (H-10)*(W-10) valid 11 x 11 windows of rint(s * 2^32) (half to even), s the
+ *                SSIM of torchmetrics' StructuralSimilarityIndexMeasure(data_range=1) at that window, evaluated in float64:
+ *                x = (double)((float)k / 255.0f); the five maps x, y, x*x, y*y, x*y filtered horizontally, then vertically,
+ *                each a sequential sum over t = 0..10 of taps[t] * v; sigma_x = E[xx] - mx*mx (no clamp), likewise sigma_y,
+ *                sigma_xy; s = ((2*(mx*my) + c1) * (2*sigma_xy + c2)) / ((mx*mx + my*my + c1) * (sigma_x + sigma_y + c2)),
+ *                c1 = 0.01^2, c2 = 0.03^2.
+ *   taps: HOST array of 11 doubles (torchmetrics' float32 Gaussian, sigma 1.5, widened).  sse, ssim_fx: [F] int64 (device),
+ *   overwritten.  IA_EINVAL: H or W < 11 (no valid window), H*W > 2^28 (the bound that keeps 3*H*W*2^32 < 2^63), F > 65535,
+ *   a row stride below 3*W, or (F > 1) a frame stride below (H-1)*row_stride + 3*W. */
+int ia_test_panel(const float* pred, const float* gt, int F, int H, int W, uint8_t* panel, ia_stream_t stream);
+int ia_image_metrics(const uint8_t* a, long frame_stride_a, long row_stride_a, const uint8_t* b, long frame_stride_b,
+                     long row_stride_b, int F, int H, int W, const double* taps, int64_t* sse, int64_t* ssim_fx,
+                     ia_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -336,6 +336,61 @@ class DNeRFModel(torch.nn.Module):
         self.global_step += 1
         return losses
 
+    def refined_batch(self, batch):
+        """DNeRF.py:74-86: when refining poses (`SMPL_param` set and `is_refine`), a copy of `batch` whose global_orient,
+        body_pose and transl (and betas for SMPLDeformer) are the refined rows SMPL_param(idx), with near / far at
+        ||transl|| -/+ 1.  The caller's tensors are not written.  Otherwise `batch` itself."""
+        if self.SMPL_param is None or not self.is_refine:
+            return batch
+        out = dict(batch)
+        idx = torch.as_tensor(batch["idx"], device=batch["rays_o"].device).reshape(-1).long()
+        with torch.no_grad():
+            body = self.SMPL_param(idx)
+        keys = ("global_orient", "body_pose", "transl") + (("betas",) if isinstance(self.deformer, SMPLDeformer) else ())
+        for k in keys[:3]:
+            if tuple(batch[k].shape) != tuple(body[k].shape):
+                raise ValueError(f"refined {k} has shape {tuple(body[k].shape)}, the batch's has {tuple(batch[k].shape)}")
+        for k in keys:
+            out[k] = body[k].detach()
+        dist = torch.norm(out["transl"], dim=-1, keepdim=True)
+        out["near"] = torch.zeros_like(batch["near"]) + (dist - 1)
+        out["far"] = torch.zeros_like(batch["far"]) + (dist + 1)
+        return out
+
+    def _split_image_shape(self, split):
+        dm = self.datamodule
+        fs = getattr(dm, f"{split}set", None) if dm is not None else None
+        if fs is None:
+            raise ValueError(f"DNeRFModel needs a datamodule with a {split}set to know the {split} image shape")
+        return tuple(fs.image_shape)
+
+    @torch.no_grad()
+    def validation_step(self, batch, batch_idx, img_size=None):
+        """DNeRF.py:171-186 without the TensorBoard images: the full frame rendered (with the refined pose when refining)
+        -> {rgb_loss, counter_avg, counter_max} as device tensors.  img_size: the valset's image shape by default."""
+        img_size = tuple(img_size) if img_size is not None else self._split_image_shape("val")
+        rgb, _, _, counter = self.render_image_fast(self.refined_batch(batch), img_size)
+        rgb_gt = batch["rgb"].reshape(-1, *img_size, 3)
+        return {"rgb_loss": (rgb - rgb_gt).square().mean(), "counter_avg": counter.mean(), "counter_max": counter.max()}
+
+    @torch.no_grad()
+    def test_step(self, batch, batch_idx, out_dir=None, img_size=None):
+        """DNeRF.py:225-239: the frame rendered (with the refined pose when refining) -> [H, 3W, 3] uint8 panel
+        [gt | pred | JET error map] in cv2's channel order (ops.test_panel).  With `out_dir` the panel is also written to
+        out_dir/{batch_idx}.png, the only copy to the host.  img_size: the testset's image shape by default."""
+        img_size = tuple(img_size) if img_size is not None else self._split_image_shape("test")
+        rgb, *_ = self.render_image_fast(self.refined_batch(batch), img_size)
+        rgb_gt = batch["rgb"].reshape(-1, *img_size, 3)
+        panel = ops.test_panel(rgb[:1].float(), rgb_gt[:1].float())[0]
+        if out_dir is not None:
+            import os
+            import cv2
+            os.makedirs(out_dir, exist_ok=True)
+            path = os.path.join(str(out_dir), f"{batch_idx}.png")
+            if not cv2.imwrite(path, panel.cpu().numpy()):
+                raise OSError(f"could not write {path}")
+        return panel
+
     @torch.no_grad()
     def render_image_sharded(self, batch, img_size, rank, world, jitters, tile=2048, peer=None):
         """One frame rendered cooperatively by `world` GPUs (BASELINE.json config 3): per-frame preparation is replicated,

@@ -755,6 +755,62 @@ def sample_patch(frames: dict, index, frame: int, num_patch: int, patch: int, ra
     return out
 
 
+def test_panel(pred, gt):
+    """DNeRF.test_step's saved image (DNeRF.py:225-239) in one launch: pred, gt [F,H,W,3] fp32 (cv2's channel order) ->
+    [F,H,3W,3] uint8 rows [q(gt) | q(pred) | JET error map] (include/ia_b200.h, ia_test_panel)"""
+    if pred.dim() != 4 or pred.shape[-1] != 3 or tuple(gt.shape) != tuple(pred.shape):
+        raise ValueError(f"test_panel: pred and gt must both be [F,H,W,3], got {tuple(pred.shape)} and {tuple(gt.shape)}")
+    F, H, W, _ = pred.shape
+    panel = torch.empty((F, H, 3 * W, 3), device=pred.device, dtype=torch.uint8)
+    _lib.count(1); check(lib().ia_test_panel(ptr(pred.contiguous(), f32), ptr(gt.contiguous(), f32), C.c_int(F), C.c_int(H),
+                                             C.c_int(W), ptr(panel), stream()))
+    return panel
+
+
+SSIM_TAPS, SSIM_SIGMA = 11, 1.5
+
+
+def ssim_taps() -> torch.Tensor:
+    """torchmetrics' `_gaussian(11, 1.5)` as eval.py's StructuralSimilarityIndexMeasure builds it: float32 on the CPU,
+    exp(-(dist / sigma)^2 / 2) normalised by its sum, returned widened to float64"""
+    dist = torch.arange((1 - SSIM_TAPS) / 2, (1 + SSIM_TAPS) / 2, step=1, dtype=torch.float32)
+    gauss = torch.exp(-torch.pow(dist / SSIM_SIGMA, 2) / 2)
+    return (gauss / gauss.sum()).double()
+
+
+def _u8_frames(t, name):
+    """(frame stride, row stride) in bytes of a uint8 [F,H,W,3] CUDA view whose pixels are 3 contiguous bytes"""
+    if not t.is_cuda:
+        raise RuntimeError("instantavatar_b200 kernels need CUDA tensors (no CPU fallback)")
+    if t.dtype != torch.uint8 or t.dim() != 4 or t.shape[-1] != 3 or t.stride(3) != 1 or t.stride(2) != 3:
+        raise ValueError(f"image_metrics: {name} must be uint8 [F,H,W,3] with contiguous pixels, got {t.dtype} "
+                         f"{tuple(t.shape)} strides {t.stride()}")
+    return t.stride(0), t.stride(1)
+
+
+def image_metrics(a, b):
+    """eval.py's per-frame PSNR and SSIM (eval.py:93-118, torchmetrics with data_range=1 on u8 / 255) from two uint8 stacks
+    [F,H,W,3] in one launch; a and b may be strided views (the pred and gt thirds of test_panel's output, decoded PNGs).
+    -> dict of psnr, ssim (float64 [F]) and the exact sums behind them, sse and ssim_fx (int64 [F]); no host synchronisation.
+    psnr = -10 log10(sse / (255^2 * 3HW)) (+inf where the images are equal); ssim = ssim_fx * 2^-32 / (3 (H-10)(W-10))."""
+    if tuple(a.shape) != tuple(b.shape):
+        raise ValueError(f"image_metrics: shapes differ, {tuple(a.shape)} and {tuple(b.shape)}")
+    fa, ra = _u8_frames(a, "a")
+    fb, rb = _u8_frames(b, "b")
+    F, H, W, _ = a.shape
+    sse = torch.empty(F, device=a.device, dtype=torch.int64)
+    ssim_fx = torch.empty(F, device=a.device, dtype=torch.int64)
+    taps = (C.c_double * SSIM_TAPS)(*ssim_taps().tolist())
+    _lib.count(1); check(lib().ia_image_metrics(C.c_void_p(a.data_ptr()), C.c_long(fa), C.c_long(ra), C.c_void_p(b.data_ptr()),
+                                                C.c_long(fb), C.c_long(rb), C.c_int(F), C.c_int(H), C.c_int(W), taps, ptr(sse),
+                                                ptr(ssim_fx), stream()))
+    # divisors as tensors: torch divides a CUDA tensor by a Python scalar through its reciprocal, which is not IEEE division
+    denom = lambda v: torch.full((F,), float(v), device=a.device, dtype=torch.float64)
+    psnr = -10.0 * torch.log10(sse.double() / denom(255.0 ** 2 * (3 * H * W)))
+    ssim = ssim_fx.double() * 2.0 ** -32 / denom(3 * (H - 10) * (W - 10))
+    return {"psnr": psnr, "ssim": ssim, "sse": sse, "ssim_fx": ssim_fx}
+
+
 # ------------------------------------------------------------------------------------------------------------------
 # device guard: every operator launches on the current stream OF THE DEVICE ITS TENSORS LIVE ON (one process may hold
 # tensors on several GPUs; function attributes and SM counts are cached per device inside the library)
