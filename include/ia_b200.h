@@ -526,6 +526,26 @@ int ia_image_metrics(const uint8_t* a, long frame_stride_a, long row_stride_a, c
                      long row_stride_b, int F, int H, int W, const double* taps, int64_t* sse, int64_t* ssim_fx,
                      ia_stream_t stream);
 
+/* GIF palettes of animation frames (animate.py:117-118, novel_view.py:127-128; DESIGN.md §3.2, §5.9).
+ *
+ * ia_gif_quantize: rgba [F][H][W][4] uint8 -> per frame f its own palette [f][256][3] (R, G, B), index [f][H][W] and
+ * n_colors[f] <= 256.  Channels (0, 1, 2) are read as R, G, B; swap_rb = 1 reads (2, 1, 0), for frames in cv2's BGRA order.
+ * Alpha is ignored.  Integer-only median cut, so results are exact:
+ *   1. histogram: per bin (r>>3, g>>3, b>>3) the pixel count and the exact channel sums;
+ *   2. one box, the bounding box (in bins) of the occupied bins;
+ *   3. while fewer than 256 boxes: take the box with the most pixels among boxes wider than one bin (ties: lowest index;
+ *      stop if none); split its longest side in bins (ties: r, g, b) at the smallest plane c in [lo, hi-1] with
+ *      2 * (pixels at or below c) >= the box's pixels (c = hi-1 if none); the lower half keeps the index, the upper half
+ *      is appended; both shrink to the bounding box of their occupied bins;
+ *   4. palette entry k = (2 * sum + n) / (2n) per channel over the box's n pixels (integer division); entries >= n_colors
+ *      are 0;
+ *   5. index = the lowest k < n_colors minimising the integer squared RGB distance to the pixel's exact colour.
+ * workspace: device, 16-byte aligned, ia_gif_quantize_workspace_bytes(F) bytes (512 KB per frame).  rgba 4-byte aligned.
+ * IA_EINVAL: F outside [0, 65535], H or W < 1, H*W > 2^24, a short workspace, a NULL pointer (F > 0). */
+size_t ia_gif_quantize_workspace_bytes(int F);
+int ia_gif_quantize(const uint8_t* rgba, int F, int H, int W, int swap_rb, uint8_t* palette, uint8_t* index, int* n_colors,
+                    void* workspace, size_t workspace_bytes, ia_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

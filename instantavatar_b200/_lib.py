@@ -30,7 +30,7 @@ SYMBOLS = [
     "ia_nv_workspace_bytes", "ia_nv_grid_build", "ia_nv_nearest", "ia_nv_pose_grad", "ia_ngp_loss",
     "ia_mc_workspace_bytes", "ia_mc_count", "ia_mc_emit", "ia_mc_component_workspace_bytes", "ia_mc_largest_component",
     "ia_skin_points", "ia_frame_index_bytes", "ia_frame_index_build", "ia_sample_edge", "ia_sample_patch",
-    "ia_test_panel", "ia_image_metrics",
+    "ia_test_panel", "ia_image_metrics", "ia_gif_quantize_workspace_bytes", "ia_gif_quantize",
 ]
 
 
@@ -80,6 +80,7 @@ def lib():
         _lib.ia_mc_workspace_bytes.restype = C.c_size_t
         _lib.ia_mc_component_workspace_bytes.restype = C.c_size_t
         _lib.ia_frame_index_bytes.restype = C.c_size_t
+        _lib.ia_gif_quantize_workspace_bytes.restype = C.c_size_t
         for s in SYMBOLS:
             getattr(_lib, s)  # fail loudly on a stale library
         if _lib.ia_abi_version() != 1:

@@ -811,6 +811,26 @@ def image_metrics(a, b):
     return {"psnr": psnr, "ssim": ssim, "sse": sse, "ssim_fx": ssim_fx}
 
 
+def gif_quantize(rgba, swap_rb: bool = False):
+    """GIF palettes of a frame stack in three launches (include/ia_b200.h, ia_gif_quantize): rgba [F,H,W,4] uint8 ->
+    (palette [F,256,3] uint8 RGB, index [F,H,W] uint8, n_colors [F] int32), one median-cut palette per frame; alpha is
+    ignored.  swap_rb: the frames are in cv2's BGRA order.  No host synchronisation."""
+    if rgba.dtype != torch.uint8 or rgba.dim() != 4 or rgba.shape[-1] != 4:
+        raise ValueError(f"gif_quantize: rgba must be uint8 [F,H,W,4], got {rgba.dtype} {tuple(rgba.shape)}")
+    F, H, W, _ = rgba.shape
+    rgba = rgba.contiguous()
+    dev = rgba.device
+    palette = torch.empty((F, 256, 3), device=dev, dtype=torch.uint8)
+    index = torch.empty((F, H, W), device=dev, dtype=torch.uint8)
+    n_colors = torch.empty(F, device=dev, dtype=torch.int32)
+    nbytes = int(lib().ia_gif_quantize_workspace_bytes(C.c_int(F)))
+    workspace = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+    _lib.count(3); check(lib().ia_gif_quantize(ptr(rgba), C.c_int(F), C.c_int(H), C.c_int(W), C.c_int(1 if swap_rb else 0),
+                                               ptr(palette), ptr(index), ptr(n_colors, torch.int32), ptr(workspace),
+                                               C.c_size_t(nbytes), stream()))
+    return palette, index, n_colors
+
+
 # ------------------------------------------------------------------------------------------------------------------
 # device guard: every operator launches on the current stream OF THE DEVICE ITS TENSORS LIVE ON (one process may hold
 # tensors on several GPUs; function attributes and SM counts are cached per device inside the library)
