@@ -906,14 +906,14 @@ __global__ void __launch_bounds__(256) adam_dev_kernel(float4* __restrict__ p, f
     if (fi == 0.f) {
         const float lr = st[0], beta1 = st[1], beta2 = st[2], eps = st[3], bc1 = st[5], bc2_sqrt = st[6], inv = st[7];
         const float step_size = lr / bc1, inv_bc2 = 1.0f / bc2_sqrt;
-        // MUFU sqrt / reciprocal (<= 2 ulp): Adam's update tolerates 1e-6 relative error
+        // IEEE sqrt: v falls below FLT_MIN for |g^| < ~1e-18, and a flushing sqrt would then drop sqrt(v) / bc2_sqrt
+        // against eps = 1e-15 (1e-3 relative in the update at step 1).  Within 14 float32 roundoffs of the float64 step
+        // (oracle/adam_ref.py, tests/test_gpu_optim.py).
         auto upd = [&](float& pp, float gg, float& mm, float& vv) {
             const float gi = gg * inv;
             mm = __fmaf_rn(beta1, mm, (1.f - beta1) * gi);
             vv = __fmaf_rn(beta2, vv, (1.f - beta2) * gi * gi);
-            float sq;
-            asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(sq) : "f"(vv));
-            pp = __fmaf_rn(-step_size, __fdividef(mm, __fmaf_rn(sq, inv_bc2, eps)), pp);
+            pp = __fmaf_rn(-step_size, __fdividef(mm, __fmaf_rn(sqrtf(vv), inv_bc2, eps)), pp);
         };
         upd(pi.x, gr.x, mi.x, vi.x); upd(pi.y, gr.y, mi.y, vi.y); upd(pi.z, gr.z, mi.z, vi.z); upd(pi.w, gr.w, mi.w, vi.w);
         __stcs(m + i, mi); __stcs(v + i, vi); __stcs(p + i, pi);
@@ -973,10 +973,8 @@ __global__ void adam_dev_tail_kernel(float* __restrict__ p, float* __restrict__ 
     const float gi = gr * inv;
     const float mm = __fmaf_rn(beta1, m[i], (1.f - beta1) * gi);
     const float vv = __fmaf_rn(beta2, v[i], (1.f - beta2) * gi * gi);
-    float sq;
-    asm("sqrt.approx.ftz.f32 %0, %1;" : "=f"(sq) : "f"(vv));
     m[i] = mm; v[i] = vv;
-    p[i] = __fmaf_rn(-(lr / bc1), __fdividef(mm, __fmaf_rn(sq, 1.0f / bc2_sqrt, eps)), p[i]);
+    p[i] = __fmaf_rn(-(lr / bc1), __fdividef(mm, __fmaf_rn(sqrtf(vv), 1.0f / bc2_sqrt, eps)), p[i]);
 }
 
 __global__ void grad_finite_kernel(const float* __restrict__ g, long n, float* __restrict__ found_inf) {
