@@ -365,13 +365,17 @@ class DNeRFModel(torch.nn.Module):
         return tuple(fs.image_shape)
 
     @torch.no_grad()
-    def validation_step(self, batch, batch_idx, img_size=None):
+    def validation_step(self, batch, batch_idx, img_size=None, return_rgb=False):
         """DNeRF.py:171-186 without the TensorBoard images: the full frame rendered (with the refined pose when refining)
-        -> {rgb_loss, counter_avg, counter_max} as device tensors.  img_size: the valset's image shape by default."""
+        -> {rgb_loss, counter_avg, counter_max} as device tensors, and with return_rgb the render itself as `rgb`
+        [1,H,W,3] (the progression image and val PSNR of train.validate).  img_size: the valset's image shape by default."""
         img_size = tuple(img_size) if img_size is not None else self._split_image_shape("val")
         rgb, _, _, counter = self.render_image_fast(self.refined_batch(batch), img_size)
         rgb_gt = batch["rgb"].reshape(-1, *img_size, 3)
-        return {"rgb_loss": (rgb - rgb_gt).square().mean(), "counter_avg": counter.mean(), "counter_max": counter.max()}
+        out = {"rgb_loss": (rgb - rgb_gt).square().mean(), "counter_avg": counter.mean(), "counter_max": counter.max()}
+        if return_rgb:
+            out["rgb"] = rgb
+        return out
 
     @torch.no_grad()
     def test_step(self, batch, batch_idx, out_dir=None, img_size=None):
