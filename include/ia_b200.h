@@ -315,8 +315,9 @@ int ia_composite_test(const float* rgb_vals, const float* sigma_vals, const floa
 
 /* Training forward.  Replaces Raymarcher.render_train (renderers/raymarcher_acc.py:140-186) together with
  * raymarch_train (raymarcher.cpp:41-53), SNARFDeformer.deform_train (snarf_deformer.py:143-159) and the network, in
- * three launches: (1) march -- one warp per ray, occupied steps become consecutive slots, their jittered posed points
- * are appended to a device-side sample list; (2) the point-query kernel over that list, every 32-sample batch an
+ * three launches: (1) march -- one warp per ray, at most 1024 steps, occupied steps become consecutive slots, their
+ * jittered posed points are appended to a device-side sample list, except those of slots whose un-jittered depth is
+ * <= 0 (near <= 0), which keep s_rgb 0, s_sigma -1e3 and s_best -1 as in :156-162; (2) the point-query kernel over that list, every 32-sample batch an
  * independent work item of all resident warps; (3) per-ray compositing.  Its time scales with the number of samples.
  * jitter [n][256] (U(0,1), replaces torch.rand_like, :158) and noise [n][256] (already scaled, replaces
  * noise*randn_like, :167) are nullable.  Outputs rgb [n][3], depth [n], alpha [n], weights [n][256] and the dense

@@ -23,13 +23,16 @@ struct TrainMarchArgs {
     const float* rays_o; const float* rays_d; const float* near; const float* far; const float* jitter;
     const uint32_t* occ_bits; const float* occ_aabb; int G;
     int n_rays;
-    float* weights; float* s_xc; float* s_z; int* s_count; int8_t* s_best;
+    float* weights; float* s_sigma; float* s_rgb; float* s_xc; float* s_z; int* s_count; int8_t* s_best;
     int* list; int* list_count;
 };
 
+constexpr int kTrainMaxSteps = 1024;  // march steps per ray (a multiple of 32), the eval render's bound (ia_kernels.cu)
+
 // one warp per ray: lane j tests steps j, j + 32, ... (t advanced by repeated addition, never as near + k * dt: the sample
 // depths equal the oracle's bit for bit), occupied steps get consecutive slots, their jittered posed points go to s_xc (the query overwrites them with
-// the canonical points), and the ray's slots are appended to the global sample list as one contiguous block
+// the canonical points), and the ray's slots in front of the origin (un-jittered depth > 0) are appended to the global
+// sample list as one contiguous block; the slots at or behind it get the reference's unqueried values here
 __global__ void __launch_bounds__(256) train_march_kernel(TrainMarchArgs a) {
     const int lane = threadIdx.x & 31;
     const int ray = blockIdx.x * (blockDim.x >> 5) + (threadIdx.x >> 5);
@@ -53,8 +56,10 @@ __global__ void __launch_bounds__(256) train_march_kernel(TrainMarchArgs a) {
         a.weights[base + s] = 0.f;
         a.s_best[base + s] = -1;
     }
-    int ray_count = 0;
-    for (;;) {
+    int ray_count = 0, n_behind = 0;
+    // at most kTrainMaxSteps steps per ray, as the eval render's march: once far - near is below ~128 ulp(near), dt is
+    // under half an ulp of t, t += dt no longer advances and an unbounded loop would never reach far
+    for (int it = 0; it < kTrainMaxSteps / 32; it++) {
         const bool act = t < far && ray_count < IA_MAX_SAMPLES;
         if (!__any_sync(kFull, act)) break;
         bool occ = false;
@@ -75,7 +80,13 @@ __global__ void __launch_bounds__(256) train_march_kernel(TrainMarchArgs a) {
             const long o = base + slot_s;
             a.s_xc[o * 3] = z * dx + ox; a.s_xc[o * 3 + 1] = z * dy + oy; a.s_xc[o * 3 + 2] = z * dz + oz;
             a.s_z[o] = z;
+            if (t <= 0.f) {  // raymarcher_acc.py:156,161-162: mask = z_vals > 0; the rest keep rgb 0, sigma -1e3 unqueried
+                a.s_sigma[o] = -1e3f;
+                a.s_rgb[o * 3] = 0.f; a.s_rgb[o * 3 + 1] = 0.f; a.s_rgb[o * 3 + 2] = 0.f;
+            }
         }
+        // t only grows, so the slots at or behind the origin are a prefix of the ray's slots
+        n_behind += __popc(__ballot_sync(kFull, occ && slot_s < IA_MAX_SAMPLES && t <= 0.f));
         ray_count += __popc(m);
         if (act) {
 #pragma unroll
@@ -83,13 +94,14 @@ __global__ void __launch_bounds__(256) train_march_kernel(TrainMarchArgs a) {
         }
     }
     const int cnt = min(ray_count, IA_MAX_SAMPLES);
+    const int n_list = cnt - n_behind;  // the slots in front of the origin go to the point query
     int first = 0;
     if (lane == 0) {
         a.s_count[ray] = cnt;
-        if (cnt > 0) first = atomicAdd(a.list_count, cnt);
+        if (n_list > 0) first = atomicAdd(a.list_count, n_list);
     }
     first = __shfl_sync(kFull, first, 0);
-    for (int s = lane; s < cnt; s += 32) a.list[first + s] = (int)(base + s);
+    for (int s = lane; s < n_list; s += 32) a.list[first + s] = (int)(base + n_behind + s);
 }
 
 struct TrainCompositeArgs {
@@ -1372,7 +1384,7 @@ int ia_train_fwd_split(const IaScene* scene, const float* rays_o, const float* r
     TrainMarchArgs m;
     m.rays_o = rays_o; m.rays_d = rays_d; m.near = near; m.far = far; m.jitter = jitter;
     m.occ_bits = reinterpret_cast<const uint32_t*>(scene->occ_bits); m.occ_aabb = scene->occ_aabb; m.G = scene->G;
-    m.n_rays = n_rays; m.weights = weights; m.s_xc = s_xc; m.s_z = s_z; m.s_count = s_count; m.s_best = s_best;
+    m.n_rays = n_rays; m.weights = weights; m.s_sigma = s_sigma; m.s_rgb = s_rgb; m.s_xc = s_xc; m.s_z = s_z; m.s_count = s_count; m.s_best = s_best;
     m.list = list; m.list_count = counters + 1;
     train_march_kernel<<<(n_rays + 7) / 8, 256, 0, st>>>(m);
     IA_CHECK_CUDA(cudaPeekAtLastError());

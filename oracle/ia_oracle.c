@@ -424,6 +424,10 @@ ORC_API void orc_ngp_forward(const float *x, long P, const float *center, const 
 /* raymarch_train: renderers/cuda/raymarcher.cu:116-161                      */
 /*  -> depths [N,N_steps] (zero-initialised here as at::zeros does, :176)    */
 /* ------------------------------------------------------------------------ */
+/* Both marches stop after ORC_MAX_MARCH_STEPS steps, as the product's do: when far - near is below ~128 ulp(near), dt is
+ * under half an ulp of t, t += dt no longer advances, and the reference's unbounded loop never reaches far. */
+#define ORC_MAX_MARCH_STEPS 1024
+
 static inline int grid_cell(float v, float c, float s, int gs) {
     return (int)clampf((v - c) * s, 0.0f, (float)gs - 1.0f);
 }
@@ -442,7 +446,7 @@ ORC_API void orc_raymarch_train(const float *rays_o, const float *rays_d, const 
         const float far = fars[n], dt = step_size[n];
         int s = 0;
         float t = nears[n];
-        while (t < far && s < N_steps) {
+        for (int k = 0; k < ORC_MAX_MARCH_STEPS && t < far && s < N_steps; k++) {
             float x = fmaf(t, dx, ox), y = fmaf(t, dy, oy), z = fmaf(t, dz, oz);
             int nx = grid_cell(x, offset[0], sx, gs), ny = grid_cell(y, offset[1], sy, gs),
                 nz = grid_cell(z, offset[2], sz, gs);
@@ -471,7 +475,7 @@ ORC_API void orc_raymarch_test(const float *rays_o, const float *rays_d, float *
         const float far = fars[n], dt = step_size[n];
         int s = 0;
         float t = nears[n];
-        while (t < far && s < N_steps) {
+        for (int k = 0; k < ORC_MAX_MARCH_STEPS && t < far && s < N_steps; k++) {
             float x = fmaf(t, dx, ox), y = fmaf(t, dy, oy), z = fmaf(t, dz, oz);
             int nx = grid_cell(x, offset[0], sx, gs), ny = grid_cell(y, offset[1], sy, gs),
                 nz = grid_cell(z, offset[2], sz, gs);

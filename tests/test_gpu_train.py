@@ -7,6 +7,7 @@ from oracle import render as orender
 from oracle import testing as scene_util
 from oracle import torch_ref
 from oracle import train_fwd_golden
+from oracle import train_fwd_ref
 
 pytestmark = pytest.mark.gpu
 
@@ -268,8 +269,8 @@ def _comp_bwd_case(seed, with_noise, with_bg, grads):
 
 
 def _comp_bwd_reference(case, dtype):
-    """d loss / d sigma [n,S] and d loss / d rgb [n,S,3] by autograd of oracle.torch_ref.composite_train in `dtype` with
-    the outputs of render_train_torch (colour + T_final * bg, white without bg; sum w*z; sum w) and
+    """d loss / d sigma [n,S] and d loss / d rgb [n,S,3] by autograd of oracle.train_fwd_ref.composite_outputs in
+    `dtype` (colour + T_final * bg, white without bg; sum w*z; sum w) and
     loss = <g_rgb, rgb> + g_depth * depth + g_alpha * alpha + <g_weights, w>.  A ray composites exactly its `count` slots.
     Also returns |d loss / d w_k| * d w_k / d sigma_k at fixed T_k: the size of the direct term that d sigma_k is the
     difference of (the other is the sample's effect on the transmittance of every later sample and the background)."""
@@ -282,10 +283,9 @@ def _comp_bwd_reference(case, dtype):
         sig = T(case["sigma"], idx, c).requires_grad_(True); col = T(case["rgb"], idx, c).requires_grad_(True)
         tot = sig + T(case["noise"], idx, c) if case["noise"] is not None else sig
         dist = torch.from_numpy(case["dt"][idx]).to(dtype)[:, None].expand(-1, c)
-        w, trans = torch_ref.composite_train(tot, dist)
         bg = torch.from_numpy(case["bg"][idx]).to(dtype) if case["bg"] is not None else torch.ones(len(idx), 3, dtype=dtype)
-        outs = {"rgb": (w[..., None] * col).sum(-2) + trans[:, -1:] * bg, "depth": (w * T(case["z"], idx, c)).sum(-1),
-                "alpha": w.sum(-1), "weights": w}
+        outs = train_fwd_ref.composite_outputs(tot, dist, col, T(case["z"], idx, c), bg)
+        w, trans = outs["weights"], outs["trans"]
         loss = sum((outs[k] * (T(gk, idx, c) if k == "weights" else torch.from_numpy(gk[idx]).to(dtype))).sum()
                    for k, gk in case["g"].items() if gk is not None)
         gs, gc, gw = torch.autograd.grad(loss, (sig, col, w), allow_unused=True, materialize_grads=True)
