@@ -59,7 +59,7 @@ typedef struct IaScene {
     const float* net_center; /* [3] NeRFNGPNet.center (ngp.py:64-71) */
     const float* net_scale;  /* [3] NeRFNGPNet.scale */
     /* [host] nullable.  Set: the deform stage is the nearest-vertex search instead of Fast-SNARF's root finding, and
-     * field / offset_k / scale_k / tfs / D / H / W are not read.  Supported by ia_render_fwd, ia_occupancy_query(_ordered),
+     * field / offset_k / scale_k / tfs / D / H / W are not read.  Supported by ia_render_fwd, ia_occupancy_query,
      * ia_deform_query and ia_train_fwd_split; ia_render_fwd_peer, ia_occupancy_query_peer, ia_broyden and ia_pose_grad
      * return IA_EINVAL (the pose gradient is ia_nv_pose_grad). */
     const IaNearestVertex* nv;
@@ -82,10 +82,10 @@ const char* ia_last_error(void);
 /* number of SMs of the current device (grid sizing is a multiple of this) [host result] */
 int ia_sm_count(void);
 
-/* tuning knobs (do not change results): "render_rays_per_warp" in {32,16,8,4,2,1}, "render_plan" in {0,1},
- * "query_warps" in {12,16,20}, "query_lanes_per_sample" in {0 = from the load, 1, 2, 4} (lanes sharing one sample's 13
- * root finds in ia_train_fwd_split's point query), "occupancy_lanes_per_point" in {0, 1, 2, 4} (the same for
- * ia_occupancy_query*; measured slower there, 0 = 1) */
+/* tuning knobs (do not change results): "render_rays_per_warp" in {4, 2, 1} (ray tile of ia_render_fwd*; the sharded
+ * frame uses 2 and 1), "query_warps" in {12, 16} (warps per CTA of ia_occupancy_query* and of ia_deform_query without
+ * xc_best, Fast-SNARF scenes), "query_lanes_per_sample" in {0 = from the load, 1, 2, 4} (lanes sharing one sample's 13 root finds in
+ * ia_train_fwd_split's point query).  Any other name is IA_EINVAL ("unknown option"). */
 int ia_set_option(const char* name, int value);
 
 /* tiny-cuda-nn HashGrid level table (models/networks/ngp.py:27-37 config). [host] outputs. */
@@ -246,17 +246,6 @@ int ia_occupancy_query(const IaScene* scene /*[host]*/, const float* jitter, con
 int ia_occupancy_query_peer(const IaScene* scene /*[host]*/, const float* jitter, const float* aabb, int G, int passes,
                             float* const* peer_density, int n_peers, void* workspace, int shard, int n_shards,
                             IaStats* stats, ia_stream_t stream);
-
-/* ia_occupancy_query / _peer with an explicit schedule.  batch_order (nullable): DEVICE list of n_order batch indices
- * (a batch = 32/passes neighbouring cells with all their passes; batch b holds cells b*(32/passes) ...), started in that
- * order by the kernel's dynamic queue; it replaces the (shard, n_shards) selection.  batch_cost (nullable): DEVICE
- * [ceil(G^3 / (32/passes))] uint32, receives the SM cycles each evaluated batch took.  Results do not depend on the order
- * (max-reduction).  With few batches per warp (a frame split over 8 GPUs: ~3) starting last frame's most expensive
- * batches first removes most of the load-balance tail.  Exactly one of density_max / peer_density is non-NULL. */
-int ia_occupancy_query_ordered(const IaScene* scene /*[host]*/, const float* jitter, const float* aabb, int G, int passes,
-                               float* density_max, float* const* peer_density, int n_peers, void* workspace, int shard,
-                               int n_shards, const int* batch_order, int n_order, unsigned* batch_cost, IaStats* stats,
-                               ia_stream_t stream);
 
 /* Measurement aid (bench.py `roofline.peak`): the fused kernels' memory access shape in isolation -- every lane gathers
  * trilinear footprints (4 x-pair records = 12 x 32-byte sectors, 12 LDG.E.256) from the L2-resident field `field`

@@ -26,7 +26,7 @@ SYMBOLS = [
     "ia_ngp_backward_scratch_bytes", "ia_adam_step", "ia_grad_check_finite", "ia_adam_prepare", "ia_adam_step_dev",
     "ia_mlp_to_half", "ia_raymarch_train", "ia_raymarch_test", "ia_composite_test", "ia_smpl_tfs", "ia_nerf_loss", "ia_pose_grad", "ia_knn1", "ia_smpl_tfs_backward", "ia_ngp_input_grad", "ia_voxelize_weights", "ia_render_fwd", "ia_deform_query", "ia_broyden", "ia_ngp_forward", "ia_transform_rays", "ia_mlp_to_half_from_half", "ia_grad_poison_shards", "ia_gather_ceiling", "ia_tcnn_backward_scratch_bytes", "ia_tcnn_encoder_forward",
     "ia_tcnn_encoder_backward", "ia_tcnn_mlp_forward", "ia_tcnn_mlp_backward", "ia_render_fwd_peer", "ia_occupancy_query_peer", "ia_peer_reduce_check",
-    "ia_peer_flags_to_found", "ia_adam_step_dev_peer", "ia_occupancy_query_ordered", "ia_train_fwd_split", "ia_train_fwd_workspace_bytes",
+    "ia_peer_flags_to_found", "ia_adam_step_dev_peer", "ia_train_fwd_split", "ia_train_fwd_workspace_bytes",
     "ia_nv_workspace_bytes", "ia_nv_grid_build", "ia_nv_nearest", "ia_nv_pose_grad", "ia_ngp_loss",
     "ia_mc_workspace_bytes", "ia_mc_count", "ia_mc_emit", "ia_mc_component_workspace_bytes", "ia_mc_largest_component",
     "ia_skin_points", "ia_frame_index_bytes", "ia_frame_index_build", "ia_sample_edge", "ia_sample_patch",

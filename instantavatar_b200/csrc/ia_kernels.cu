@@ -10,11 +10,11 @@
 
 using namespace ia;
 
-static int g_render_rays = 4;  // rays per warp (32 / 16 / 8 / 4), tunable through ia_set_option
-static int g_render_plan = 1;  // longest-first tile scheduling (needs the large workspace)
-static int g_query_warps = 12;   // same for the point-query kernel (12 / 16 / 20; 16 and 20 only without xc output)
+static int g_render_rays = 4;  // rays per warp of the renderer (4 / 2 / 1; the sharded frame uses 2 and 1), ia_set_option
+static int g_query_warps = 12;  // warps per CTA of the point query without xc output (12 / 16), ia_set_option
 static int g_query_lanes = 0;  // lanes per point of the list-mode point query (training forward): 0 = auto, 1 / 2 / 4
-static int g_occ_lanes = 0;    // lanes per point of the occupancy passes: 0 = 1 (more were measured slower, see occupancy_query_impl)
+
+constexpr int kRenderWarps = 12;  // warps per CTA of the fused renderer (one CTA per SM)
 
 #include "ia_host.h"
 #include "ia_scene.cuh"
@@ -54,14 +54,14 @@ struct RenderWarpExtra {
 };
 
 // kNV: nearest-vertex deform stage (warp_eval_nv), one candidate per sample
-template <int kWarps, bool kNV = false>
+template <bool kNV = false>
 struct RenderSmem {
     __align__(128) uint32_t occ[64 * 64 * 64 / 32];
     __align__(16) __half W[kMlpHalfs];
     FrameConst fc;
     __align__(8) uint64_t mbar;
-    std::conditional_t<kNV, WarpScratchNV, WarpScratch<false>> ws[kWarps];
-    RenderWarpExtra wx[kWarps];
+    std::conditional_t<kNV, WarpScratchNV, WarpScratch<false>> ws[kRenderWarps];
+    RenderWarpExtra wx[kRenderWarps];
 };
 
 // Conservative parametric interval of the ray inside the bounding box of the OCCUPIED cells (cell box from
@@ -89,9 +89,12 @@ __device__ __forceinline__ void occupied_interval(const FrameConst& fc, const in
     }
 }
 
+// a warp's kRays rays (4 / 2 / 1) form a tile_width x (kRays / tile_width) block of pixels when the frame is tiled
+__host__ __device__ constexpr int tile_width(int rays) { return rays >= 2 ? 2 : 1; }
+
 template <int kRays>
 __device__ __forceinline__ int tile_ray(int tile, int rl, bool tiled, int image_width) {
-    constexpr int kTileW = kRays == 32 ? 8 : (kRays >= 8 ? 4 : (kRays >= 2 ? 2 : 1));
+    constexpr int kTileW = tile_width(kRays);
     if (tiled) {
         const int tiles_x = image_width / kTileW;
         const int ty = tile / tiles_x, tx = tile % tiles_x;
@@ -108,7 +111,7 @@ __global__ void __launch_bounds__(256) render_plan_kernel(const __grid_constant_
     __shared__ FrameConst fc;
     load_frame_const<kNV>(fc, a.sd);
     __syncthreads();
-    constexpr int kTileW = kRays == 32 ? 8 : (kRays >= 8 ? 4 : (kRays >= 2 ? 2 : 1));
+    constexpr int kTileW = tile_width(kRays);
     constexpr int kTileH = kRays / kTileW;
     const int G = a.sd.s.G;
     const uint32_t* occ = a.sd.s.occ_bits;
@@ -204,13 +207,13 @@ __global__ void __launch_bounds__(1024) order_tiles_kernel(const int* __restrict
 // kRays rays per warp, each marched kDepth = 32/kRays steps ahead (lane = depth * kRays + ray): the batch of 32
 // samples a warp evaluates stays spatially coherent (neighbouring pixels x consecutive steps) while the number of
 // independent work units grows by kDepth -- there are fewer hit rays in a 512^2 frame than resident lanes.
-template <int kWarps, int kRays, bool kNV = false>
-__global__ void __launch_bounds__(kWarps * 32, 1) render_fwd_kernel(const __grid_constant__ RenderArgs a) {
+template <int kRays, bool kNV = false>
+__global__ void __launch_bounds__(kRenderWarps * 32, 1) render_fwd_kernel(const __grid_constant__ RenderArgs a) {
     constexpr int kDepth = 32 / kRays;
-    constexpr int kTileW = kRays == 32 ? 8 : (kRays >= 8 ? 4 : (kRays >= 2 ? 2 : 1));
+    constexpr int kTileW = tile_width(kRays);
     constexpr int kTileH = kRays / kTileW;
     extern __shared__ __align__(128) unsigned char smem_raw[];
-    RenderSmem<kWarps, kNV>& sm = *reinterpret_cast<RenderSmem<kWarps, kNV>*>(smem_raw);
+    RenderSmem<kNV>& sm = *reinterpret_cast<RenderSmem<kNV>*>(smem_raw);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int G = a.sd.s.G;
     // ---- prologue: TMA-engine bulk copies of the occupancy bitfield and the MLP weights -------------
@@ -396,10 +399,6 @@ struct QueryArgs {
     int* batch_counter;  // optional: dynamic batch scheduling (zeroed by the launcher)
     int batch_first, batch_stride;  // grid mode: this launch handles batches first, first+stride, ... (multi-GPU sharding)
     float* const* peer_density; int n_peers;  // grid mode over peer memory: max-reduce into EVERY rank's density (NVLink atomics)
-    // grid mode, optional: an explicit list of the batches of this launch in the order they should be started (longest
-    // first removes the load-balance tail when a rank holds only a few batches per warp), and the measured cost of each
-    // batch (SM cycles) that the next frame's order can be built from
-    const int* batch_order; int n_order; unsigned* batch_cost;
     // point mode, optional (split training forward, ia_train.cu): the number of points lives on the device (n = capacity)
     // and point p reads pts / writes every output at element index[p] instead of p
     const int* n_dev; const int* index;
@@ -415,11 +414,10 @@ struct QuerySmem {
 };
 
 // kKeepXc: the canonical point of the winning candidate is an output (xc_best; training-time queries); the occupancy
-// passes do not need it, which frees 5 KB of shared memory per warp => more resident warps per SM
-// kDynLanes: lanes per point chosen at run time (a.lanes_per_sample); the default occupancy-pass instantiation keeps the
-// one-lane-per-point code with a literal 1
+// passes do not need it, which frees 5 KB of shared memory per warp.  Fast-SNARF queries that keep it choose the lanes
+// per point at run time (a.lanes_per_sample); the occupancy passes run one lane per point with a literal 1
 // kNV: nearest-vertex deform stage (warp_eval_nv, one lane per point)
-template <int kWarps, bool kKeepXc, bool kDynLanes = kKeepXc, bool kNV = false>
+template <int kWarps, bool kKeepXc, bool kNV = false>
 __global__ void __launch_bounds__(kWarps * 32, 1) deform_query_kernel(const __grid_constant__ QueryArgs a) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     QuerySmem<kWarps, kKeepXc, kNV>& sm = *reinterpret_cast<QuerySmem<kWarps, kKeepXc, kNV>*>(smem_raw);
@@ -445,7 +443,7 @@ __global__ void __launch_bounds__(kWarps * 32, 1) deform_query_kernel(const __gr
     // with few points per resident warp a batch's latency (13 serial root finds per lane) is the kernel's time; k lanes per
     // point divide it (warp_eval_samples) at no extra memory traffic.  Point mode, k = 0: about one batch per warp.
     int k = 1;
-    if (kDynLanes) {
+    if (kKeepXc && !kNV) {
         k = a.lanes_per_sample;
         if (k == 0) {
             const int n_warps = gridDim.x * kWarps, n32 = (n_pts + 31) / 32;
@@ -461,13 +459,8 @@ __global__ void __launch_bounds__(kWarps * 32, 1) deform_query_kernel(const __gr
             if (lane == 0) nb = atomicAdd(a.batch_counter, 1);
             lidx = __shfl_sync(kFull, nb, 0);
         }
-        int bidx = a.batch_first + lidx * a.batch_stride;
-        if (a.batch_order) {
-            if (lidx >= a.n_order) break;
-            bidx = a.batch_order[lidx];
-        }
+        const int bidx = a.batch_first + lidx * a.batch_stride;
         if (bidx >= n_batches || bidx < 0) break;
-        const long long t_start = a.batch_cost ? clock64() : 0;
         int p = bidx * spw + (lane & (spw - 1));
         bool act = p < n_pts;
         const bool owner = lane < spw;  // helper lanes (k > 1) evaluate some of their point's root finds, nothing else
@@ -499,7 +492,7 @@ __global__ void __launch_bounds__(kWarps * 32, 1) deform_query_kernel(const __gr
         SampleOut so;
         if constexpr (kNV) {
             warp_eval_nv(ctx, a.sd.nv, sm.ws[warp], act, x, y, z, a.eval_mode != 0, lane, so, st_roots, st_hash);
-        } else if constexpr (kDynLanes) {
+        } else if constexpr (kKeepXc) {
             warp_eval_samples<kKeepXc>(ctx, sm.ws[warp], act, x, y, z, a.eval_mode != 0, lane, so, st_gather, st_roots, st_load, st_hash, k);
         } else {
             warp_eval_samples<kKeepXc>(ctx, sm.ws[warp], act, x, y, z, a.eval_mode != 0, lane, so, st_gather, st_roots, st_load, st_hash);
@@ -523,10 +516,6 @@ __global__ void __launch_bounds__(kWarps * 32, 1) deform_query_kernel(const __gr
                 if (a.xc_best) { a.xc_best[q * 3] = so.xc[0]; a.xc_best[q * 3 + 1] = so.xc[1]; a.xc_best[q * 3 + 2] = so.xc[2]; }
             }
             if (a.best_init) a.best_init[q] = (int8_t)so.best;
-        }
-        if (a.batch_cost) {
-            __syncwarp();
-            if (lane == 0) a.batch_cost[bidx] = (unsigned)min((long long)0xffffffffll, clock64() - t_start);
         }
     }
     if (a.stats) {
@@ -873,28 +862,13 @@ int ia_sm_count(void) { return sm_count(); }
 int ia_set_option(const char* name, int value) {
     IA_REQUIRE(name != nullptr);
     if (!strcmp(name, "render_rays_per_warp")) {
-        IA_REQUIRE(value == 32 || value == 16 || value == 8 || value == 4 || value == 2 || value == 1);
+        IA_REQUIRE(value == 4 || value == 2 || value == 1);
         g_render_rays = value;
         return IA_OK;
     }
-    if (!strcmp(name, "render_plan")) {
-        g_render_plan = value != 0;
-        return IA_OK;
-    }
-    if (!strcmp(name, "render_warps")) {
-        // 12 only: the 16-warp build (128 registers) does not fit next to the staged hash level; the name stays so that
-        // callers passing other values fail loudly
-        IA_REQUIRE(value == 12);
-        return IA_OK;
-    }
     if (!strcmp(name, "query_warps")) {
-        IA_REQUIRE(value == 12 || value == 16 || value == 20);
+        IA_REQUIRE(value == 12 || value == 16);
         g_query_warps = value;
-        return IA_OK;
-    }
-    if (!strcmp(name, "occupancy_lanes_per_point")) {
-        IA_REQUIRE(value == 0 || value == 1 || value == 2 || value == 4);
-        g_occ_lanes = value;
         return IA_OK;
     }
     if (!strcmp(name, "query_lanes_per_sample")) {
@@ -972,18 +946,18 @@ size_t ia_render_workspace_bytes(int n_rays) { return 256 + 2 * sizeof(int) * (s
 
 }  // extern "C"
 
-template <int kWarps, int kRays, bool kNV = false>
+template <int kRays, bool kNV = false>
 static int launch_render(RenderArgs& a, bool plan, int* ws_cost, int* ws_order, cudaStream_t st) {
-    const size_t smem = sizeof(RenderSmem<kWarps, kNV>);
+    const size_t smem = sizeof(RenderSmem<kNV>);
     static PerDeviceFlag attr_set;
     if (!attr_set.get()) {
-        IA_CHECK_CUDA(cudaFuncSetAttribute(render_fwd_kernel<kWarps, kRays, kNV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        IA_CHECK_CUDA(cudaFuncSetAttribute(render_fwd_kernel<kRays, kNV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set.set();
     }
     const int n_tiles = (a.n_rays + kRays - 1) / kRays;
     int grid = sm_count();
     if (grid <= 0) return set_err(IA_ECUDA, "no CUDA device%s");
-    grid = min(grid, (n_tiles + kWarps - 1) / kWarps);
+    grid = min(grid, (n_tiles + kRenderWarps - 1) / kRenderWarps);
     if (plan) {
         const long threads = (long)n_tiles * kRays;
         render_plan_kernel<kRays, kNV><<<(unsigned)((threads + 255) / 256), 256, 0, st>>>(a, ws_cost);
@@ -991,40 +965,37 @@ static int launch_render(RenderArgs& a, bool plan, int* ws_cost, int* ws_order, 
         a.tile_order = ws_order;
         a.n_active = a.tile_counter + 1;
     }
-    render_fwd_kernel<kWarps, kRays, kNV><<<grid, kWarps * 32, smem, st>>>(a);
+    render_fwd_kernel<kRays, kNV><<<grid, kRenderWarps * 32, smem, st>>>(a);
     return IA_OK;
 }
 
-template <int kWarps, bool kKeepXc, bool kDynLanes = kKeepXc, bool kNV = false>
+template <int kWarps, bool kKeepXc, bool kNV = false>
 static int launch_query_t(QueryArgs& a, cudaStream_t stream) {
     const size_t smem = sizeof(QuerySmem<kWarps, kKeepXc, kNV>);
     static PerDeviceFlag attr_set;
     if (!attr_set.get()) {
-        IA_CHECK_CUDA(cudaFuncSetAttribute(deform_query_kernel<kWarps, kKeepXc, kDynLanes, kNV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
+        IA_CHECK_CUDA(cudaFuncSetAttribute(deform_query_kernel<kWarps, kKeepXc, kNV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set.set();
     }
     const int n_batches = a.grid_aabb ? (a.G * a.G * a.G + (32 / a.passes) - 1) / (32 / a.passes) : (a.n + 31) / 32;
     int grid = sm_count();
     if (grid <= 0) return set_err(IA_ECUDA, "no CUDA device%s");
     grid = min(grid, (n_batches + kWarps - 1) / kWarps);
-    deform_query_kernel<kWarps, kKeepXc, kDynLanes, kNV><<<grid, kWarps * 32, smem, stream>>>(a);
+    deform_query_kernel<kWarps, kKeepXc, kNV><<<grid, kWarps * 32, smem, stream>>>(a);
     IA_CHECK_CUDA(cudaPeekAtLastError());
     return IA_OK;
 }
 
 static int launch_query(QueryArgs& a, cudaStream_t stream) {
-    if (a.sd.s.nv) {  // nearest-vertex deformer: one lane per point, default launch shape
+    if (a.sd.s.nv) {  // nearest-vertex deformer: one lane per point
         a.lanes_per_sample = 1;
-        if (a.xc_best) return launch_query_t<12, true, false, true>(a, stream);
-        return launch_query_t<12, false, false, true>(a, stream);
+        if (a.xc_best) return launch_query_t<12, true, true>(a, stream);
+        return launch_query_t<12, false, true>(a, stream);
     }
     if (a.xc_best) return launch_query_t<12, true>(a, stream);
-    if (a.grid_aabb && a.lanes_per_sample > 1) return launch_query_t<12, false, true>(a, stream);  // narrow occupancy batches
-    switch (g_query_warps) {
-        case 20: return launch_query_t<20, false>(a, stream);
-        case 16: return launch_query_t<16, false>(a, stream);
-        default: return launch_query_t<12, false>(a, stream);
-    }
+    // 16 warps measured ~1 % faster than 12 for the occupancy passes on an H100 (DESIGN §5.2); the default is still 12
+    if (g_query_warps == 16) return launch_query_t<16, false>(a, stream);
+    return launch_query_t<12, false>(a, stream);
 }
 
 extern "C" {
@@ -1050,24 +1021,19 @@ static int render_fwd_impl(const IaScene* scene, const float* rays_o, const floa
     cudaStream_t st = (cudaStream_t)stream;
     IA_CHECK_CUDA(cudaMemsetAsync(workspace, 0, 256, st));
     // with a large enough workspace the tiles are scheduled longest-first (removes the load-balance tail)
-    const bool plan = g_render_plan && workspace_bytes >= ia_render_workspace_bytes(n_rays);
+    const bool plan = workspace_bytes >= ia_render_workspace_bytes(n_rays);
     int* ws_cost = reinterpret_cast<int*>(reinterpret_cast<char*>(workspace) + 256);
     int* ws_order = ws_cost + (n_rays + 1);
-    const int rpw = g_render_rays;
     if (scene->nv) {  // nearest-vertex deformer: the default tile shape (results do not depend on it)
-        rc = launch_render<12, 4, true>(a, plan, ws_cost, ws_order, st);
+        rc = launch_render<4, true>(a, plan, ws_cost, ws_order, st);
         if (rc) return rc;
         IA_CHECK_CUDA(cudaPeekAtLastError());
         return IA_OK;
     }
-    // (a 16-warp renderer no longer fits next to the staged hash level)
-    switch (rpw) {
-        case 32: rc = launch_render<12, 32>(a, plan, ws_cost, ws_order, st); break;
-        case 16: rc = launch_render<12, 16>(a, plan, ws_cost, ws_order, st); break;
-        case 4: rc = launch_render<12, 4>(a, plan, ws_cost, ws_order, st); break;
-        case 2: rc = launch_render<12, 2>(a, plan, ws_cost, ws_order, st); break;
-        case 1: rc = launch_render<12, 1>(a, plan, ws_cost, ws_order, st); break;
-        default: rc = launch_render<12, 8>(a, plan, ws_cost, ws_order, st); break;
+    switch (g_render_rays) {
+        case 2: rc = launch_render<2>(a, plan, ws_cost, ws_order, st); break;
+        case 1: rc = launch_render<1>(a, plan, ws_cost, ws_order, st); break;
+        default: rc = launch_render<4>(a, plan, ws_cost, ws_order, st); break;
     }
     if (rc) return rc;
     IA_CHECK_CUDA(cudaPeekAtLastError());
@@ -1104,7 +1070,6 @@ int ia_deform_query(const IaScene* scene, const float* pts, int n, int eval_mode
     a.grid_jitter = nullptr; a.grid_aabb = nullptr; a.G = 0; a.density_max = nullptr; a.passes = 1;
     a.batch_counter = nullptr; a.batch_first = 0; a.batch_stride = 1;
     a.peer_density = nullptr; a.n_peers = 0;
-    a.batch_order = nullptr; a.n_order = 0; a.batch_cost = nullptr;
     a.n_dev = nullptr; a.index = nullptr; a.lanes_per_sample = 1;
     return launch_query(a, (cudaStream_t)stream);
 }
@@ -1125,15 +1090,13 @@ __attribute__((visibility("hidden"))) int ia_internal_query_list(const IaScene* 
     a.grid_jitter = nullptr; a.grid_aabb = nullptr; a.G = 0; a.density_max = nullptr; a.passes = 1;
     a.batch_counter = batch_counter; a.batch_first = 0; a.batch_stride = 1;
     a.peer_density = nullptr; a.n_peers = 0;
-    a.batch_order = nullptr; a.n_order = 0; a.batch_cost = nullptr;
     a.n_dev = n_dev; a.index = index; a.lanes_per_sample = g_query_lanes;
     return launch_query(a, (cudaStream_t)stream);
 }
 
 static int occupancy_query_impl(const IaScene* scene, const float* jitter, const float* aabb, int G, int passes,
                                 float* density_max, float* const* peer_density, int n_peers, void* workspace, int shard,
-                                int n_shards, IaStats* stats, ia_stream_t stream, const int* batch_order = nullptr,
-                                int n_order = 0, unsigned* batch_cost = nullptr) {
+                                int n_shards, IaStats* stats, ia_stream_t stream) {
     IA_REQUIRE(jitter && aabb && (density_max || peer_density) && G > 0 && passes > 0 && passes <= 32);
     IA_REQUIRE(n_shards >= 1 && shard >= 0 && shard < n_shards);
     QueryArgs a;
@@ -1145,14 +1108,11 @@ static int occupancy_query_impl(const IaScene* scene, const float* jitter, const
     a.batch_counter = reinterpret_cast<int*>(workspace);
     a.batch_first = shard; a.batch_stride = n_shards;
     a.peer_density = peer_density; a.n_peers = n_peers;
-    a.batch_order = batch_order; a.n_order = n_order; a.batch_cost = batch_cost;
     a.n_dev = nullptr; a.index = nullptr;
-    // several lanes per point ("occupancy_lanes_per_point") were measured and do NOT pay here, unlike in the training list
-    // query: 98 % of the grid points are empty space whose solves end after one or two gathers, so splitting a point's 13
-    // solves over lanes shortens nothing and idles the helper lanes in every later stage.  Default 1.
-    a.lanes_per_sample = g_occ_lanes ? g_occ_lanes : 1;
-    if (batch_order || batch_cost || 32 / a.lanes_per_sample < passes) a.lanes_per_sample = 1;
-    IA_REQUIRE(!batch_order || (workspace && n_order >= 0));
+    // one lane per point: unlike in the training list query, several lanes per point do not pay here -- 98 % of the grid
+    // points are empty space whose solves end after one or two gathers, so splitting a point's 13 solves over lanes
+    // shortens nothing and idles the helper lanes in every later stage
+    a.lanes_per_sample = 1;
     if (workspace) IA_CHECK_CUDA(cudaMemsetAsync(workspace, 0, 256, (cudaStream_t)stream));
     // peer mode: every rank's buffer is written by all ranks -- the CALLER zeroes it (before the barrier that precedes this launch)
     if (!peer_density) IA_CHECK_CUDA(cudaMemsetAsync(density_max, 0, sizeof(float) * G * G * G, (cudaStream_t)stream));
@@ -1171,17 +1131,6 @@ extern "C" int ia_occupancy_query_peer(const IaScene* scene, const float* jitter
     IA_REJECT_NV(scene, "ia_occupancy_query_peer");
     IA_REQUIRE(peer_density && n_peers >= 1 && n_peers <= 64);
     return occupancy_query_impl(scene, jitter, aabb, G, passes, nullptr, peer_density, n_peers, workspace, shard, n_shards, stats, stream);
-}
-
-extern "C" int ia_occupancy_query_ordered(const IaScene* scene, const float* jitter, const float* aabb, int G, int passes,
-                                          float* density_max, float* const* peer_density, int n_peers, void* workspace,
-                                          int shard, int n_shards, const int* batch_order, int n_order,
-                                          unsigned* batch_cost, IaStats* stats, ia_stream_t stream) {
-    IA_REQUIRE((density_max != nullptr) != (peer_density != nullptr));
-    if (peer_density) IA_REJECT_NV(scene, "ia_occupancy_query_ordered over peer memory");
-    IA_REQUIRE(!peer_density || (n_peers >= 1 && n_peers <= 64));
-    return occupancy_query_impl(scene, jitter, aabb, G, passes, density_max, peer_density, n_peers, workspace, shard, n_shards,
-                                stats, stream, batch_order, n_order, batch_cost);
 }
 
 int ia_broyden(const IaScene* scene, const float* xd, int n, float* xc, uint8_t* valid, float* j_inv, ia_stream_t stream) {

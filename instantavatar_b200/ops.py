@@ -113,35 +113,14 @@ def mc_largest_component(verts: torch.Tensor, faces: torch.Tensor):
     return verts_out[:kv], faces_out[:kf]
 
 
-def occupancy_batches(G: int, passes: int) -> int:
-    """number of scheduling batches of the occupancy query (32 // passes neighbouring cells with all their passes each)"""
-    cpb = 32 // passes
-    return (G ** 3 + cpb - 1) // cpb
-
-
-def occupancy_query(scene, jitters: torch.Tensor, aabb6: torch.Tensor, density=None, stats=None, workspace=None, shard=(0, 1), peer=None,
-                    order=None, cost=None):
+def occupancy_query(scene, jitters: torch.Tensor, aabb6: torch.Tensor, density=None, stats=None, workspace=None, shard=(0, 1), peer=None):
     """5-pass density query of DensityGrid.initialize in one launch -> density [G,G,G] (max over passes, >= 0).
     peer = (device address of the array of every rank's density pointer, n_ranks): this rank's shard is max-reduced into
-    all ranks' (pre-zeroed) buffers with NVLink atomics; returns None (the caller owns the symmetric buffer).
-    order (int32 [k], device): explicit list of batches to evaluate, in start order (replaces `shard`);
-    cost (int32 [occupancy_batches], device): receives the SM cycles of every evaluated batch."""
+    all ranks' (pre-zeroed) buffers with NVLink atomics; returns None (the caller owns the symmetric buffer)."""
     P, G = jitters.shape[0], jitters.shape[1]
     if workspace is None:
         workspace = torch.empty(64, device=jitters.device, dtype=torch.int32)
     s = scene.c_struct()
-    if order is not None or cost is not None:
-        assert order is None or (order.dtype == torch.int32 and order.is_contiguous())
-        assert cost is None or (cost.dtype == torch.int32 and cost.numel() >= occupancy_batches(G, P))
-        if peer is None and density is None:
-            density = torch.empty((G, G, G), device=jitters.device, dtype=f32)
-        _lib.count(1); check(lib().ia_occupancy_query_ordered(
-            C.byref(s), ptr(jitters.contiguous(), f32), ptr(aabb6, f32), C.c_int(G), C.c_int(P),
-            ptr(density) if peer is None else None, C.c_void_p(int(peer[0])) if peer is not None else None,
-            C.c_int(int(peer[1]) if peer is not None else 0), ptr(workspace), C.c_int(shard[0]), C.c_int(shard[1]),
-            ptr(order) if order is not None else None, C.c_int(order.numel() if order is not None else 0),
-            ptr(cost) if cost is not None else None, ptr(stats), stream()))
-        return None if peer is not None else density
     if peer is not None:
         _lib.count(1); check(lib().ia_occupancy_query_peer(C.byref(s), ptr(jitters.contiguous(), f32), ptr(aabb6, f32), C.c_int(G), C.c_int(P),
                                                            C.c_void_p(int(peer[0])), C.c_int(int(peer[1])), ptr(workspace), C.c_int(shard[0]),
@@ -252,19 +231,18 @@ def gather_ceiling(field: torch.Tensor, iters: int = 200, warps: int = 12, coher
 
 
 # the library's tuning knobs (ia_set_option) and their defaults, mirrored here so that a caller can change one temporarily
-_OPTIONS = {"render_rays_per_warp": 4, "render_plan": 1, "render_warps": 12, "query_warps": 12,
-            "query_lanes_per_sample": 0, "occupancy_lanes_per_point": 0}
-# options of the retired one-kernel training forward, still readable (bench.py reports them) at the only value the
-# three-launch forward has: it is always the forward (train_split) and runs one warp per ray (train_rays_per_warp)
-_FIXED_OPTIONS = {"train_split": 1, "train_rays_per_warp": 1}
+_OPTIONS = {"render_rays_per_warp": 4, "query_warps": 12, "query_lanes_per_sample": 0}
+# retired options, still readable (bench.py reports and sets them) at the one value the kernels have: the three-launch
+# training forward (train_split) with one warp per ray (train_rays_per_warp), and 12 warps per CTA in the fused renderer
+# (render_warps)
+_FIXED_OPTIONS = {"train_split": 1, "train_rays_per_warp": 1, "render_warps": 12}
 _train_ws: dict = {}
 
 
 def set_option(name: str, value: int):
     if name in _FIXED_OPTIONS:
         if int(value) != _FIXED_OPTIONS[name]:
-            raise ValueError(f"{name} can only be {_FIXED_OPTIONS[name]}: the one-kernel training forward it configured "
-                             "was retired")
+            raise ValueError(f"{name} can only be {_FIXED_OPTIONS[name]}: the other kernels it selected were retired")
         return
     check(lib().ia_set_option(name.encode(), C.c_int(value)))
     _OPTIONS[name] = int(value)

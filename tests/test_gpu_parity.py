@@ -230,8 +230,8 @@ def test_occupancy_build_matches_oracle(sc, dev):
     np.testing.assert_array_equal(f2.cpu().numpy(), g["grid/field"])
 
 
-def test_render_all_warp_shapes_agree(sc, dev):
-    """the rays-per-warp tuning knob must not change results"""
+def test_render_every_ray_tile_agrees(sc, dev):
+    """the rays-per-warp tuning knob (4 / 2 / 1, tiled and untiled) must not change results"""
     import torch
     from instantavatar_b200 import ops
     scene, _ = dev
@@ -241,7 +241,7 @@ def test_render_all_warp_shapes_agree(sc, dev):
     idx = (ys[:, None] * 512 + xs[None]).ravel()
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a[idx])).cuda()
     outs = []
-    for rpw in (32, 16, 8, 4, 2, 1):
+    for rpw in (4, 2, 1):
         ops.set_option("render_rays_per_warp", rpw)
         for w in (96, 0):
             out = ops.render_fwd(scene, t(o), t(d), t(near), t(far), None, w)
@@ -252,9 +252,9 @@ def test_render_all_warp_shapes_agree(sc, dev):
             np.testing.assert_array_equal(o2[k], outs[0][k])
 
 
-def test_occupancy_query_shards_and_explicit_order_reproduce_the_grid(sc, dev):
-    """ia_occupancy_query_ordered: strided shards and explicit batch lists (any order, any partition) max-reduce to the
-    bits of the single launch; the per-batch cycle counts cover every batch."""
+def test_occupancy_query_shards_reproduce_the_grid(sc, dev):
+    """strided shards of ia_occupancy_query max-reduce to the bits of the single launch; so
+    does the 16-warp launch"""
     import torch
     from instantavatar_b200 import ops
     scene, _ = dev
@@ -262,37 +262,14 @@ def test_occupancy_query_shards_and_explicit_order_reproduce_the_grid(sc, dev):
     t = lambda a: torch.from_numpy(np.ascontiguousarray(a)).cuda()
     jit = t(sc["occ_jitter"])
     aabb = t(fr["bbox_deformed"].reshape(6))
-    P, G = jit.shape[0], jit.shape[1]
-    nb = ops.occupancy_batches(G, P)
-    cost = torch.zeros(nb, dtype=torch.int32, device="cuda")
     full = ops.occupancy_query(scene, jit, aabb).clone()
-    with_cost = ops.occupancy_query(scene, jit, aabb, cost=cost).clone()
-    assert torch.equal(full, with_cost)
-    assert int((cost > 0).sum()) == nb
-    acc = torch.zeros_like(full)
-    for r in range(3):
-        acc = torch.maximum(acc, ops.occupancy_query(scene, jit, aabb, shard=(r, 3)))
-    assert torch.equal(acc, full)
-    g = torch.Generator(device="cpu"); g.manual_seed(5)
-    perm = torch.randperm(nb, generator=g).to(torch.int32).cuda()
-    by_cost = torch.argsort(cost, descending=True).to(torch.int32)
-    acc = torch.zeros_like(full)
-    for part in (perm[: nb // 3], perm[nb // 3:]):
-        acc = torch.maximum(acc, ops.occupancy_query(scene, jit, aabb, order=part.contiguous()))
-    assert torch.equal(acc, full)
-    assert torch.equal(ops.occupancy_query(scene, jit, aabb, order=by_cost.contiguous()), full)
-    # narrow batches (2 / 4 lanes share a point's 13 root finds; an option, off by default: measured slower for these passes)
-    try:
-        for k in (2, 4):
-            ops.set_option("occupancy_lanes_per_point", k)
-            assert torch.equal(ops.occupancy_query(scene, jit, aabb), full), k
-            acc = torch.zeros_like(full)
-            for r in range(4):
-                acc = torch.maximum(acc, ops.occupancy_query(scene, jit, aabb, shard=(r, 4)))
-            assert torch.equal(acc, full), k
+    for n_shards in (3, 4):
+        acc = torch.zeros_like(full)
+        for r in range(n_shards):
+            acc = torch.maximum(acc, ops.occupancy_query(scene, jit, aabb, shard=(r, n_shards)))
+        assert torch.equal(acc, full), n_shards
+    try:   # the 16-warp launch shape
+        ops.set_option("query_warps", 16)
+        assert torch.equal(ops.occupancy_query(scene, jit, aabb), full)
     finally:
-        ops.set_option("occupancy_lanes_per_point", 0)
-    acc = torch.zeros_like(full)
-    for r in range(4):   # default policy at 4 shards
-        acc = torch.maximum(acc, ops.occupancy_query(scene, jit, aabb, shard=(r, 4)))
-    assert torch.equal(acc, full)
+        ops.set_option("query_warps", 12)

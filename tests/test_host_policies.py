@@ -17,27 +17,37 @@ def test_shard_layout_covers_and_aligns():
             assert L - n < world * 64 + 64                       # padding stays small
 
 
-def test_option_mirror_defaults_match_the_library_defaults():
+def test_option_mirror_matches_the_library_and_refuses_retired_options():
     import ctypes
     import re
     import os
     import pytest
     from instantavatar_b200 import _lib, ops
     src = open(os.path.join(os.path.dirname(ops.__file__), "csrc", "ia_kernels.cu")).read()
-    for name, var in (("render_rays_per_warp", "g_render_rays"), ("render_plan", "g_render_plan"), ("query_warps", "g_query_warps"),
-                      ("query_lanes_per_sample", "g_query_lanes"), ("occupancy_lanes_per_point", "g_occ_lanes")):
+    for name, var in (("render_rays_per_warp", "g_render_rays"), ("query_warps", "g_query_warps"),
+                      ("query_lanes_per_sample", "g_query_lanes")):
         m = re.search(r"static int %s = (\d+);" % var, src)
         assert m and int(m.group(1)) == ops._OPTIONS[name], name
-    # the retired one-kernel training forward's options: readable and settable at their one value, never the library's
-    for name in ("train_split", "train_rays_per_warp"):
-        assert ops.get_option(name) == 1
-        ops.set_option(name, 1)
-        for value in (0, 2, 4):
-            with pytest.raises(ValueError, match="retired"):
-                ops.set_option(name, value)
-        assert ops.get_option(name) == 1
-    assert _lib.lib().ia_set_option(b"train_rays_per_warp", ctypes.c_int(1)) == -1
-    assert b"unknown option" in _lib.lib().ia_last_error()
+    assert set(ops._OPTIONS) == {"render_rays_per_warp", "query_warps", "query_lanes_per_sample"}
+    # retired options: readable and settable at their one value, never the library's
+    for name, one in (("train_split", 1), ("train_rays_per_warp", 1), ("render_warps", 12)):
+        assert ops.get_option(name) == one
+        ops.set_option(name, one)
+        for value in (0, 1, 2, 4, 8, 16, 20):
+            if value != one:
+                with pytest.raises(ValueError, match="retired"):
+                    ops.set_option(name, value)
+        assert ops.get_option(name) == one
+    # ... and unknown to the library, even at the value it used to default to
+    for name, value in ((b"train_rays_per_warp", 1), (b"render_plan", 1), (b"occupancy_lanes_per_point", 0),
+                        (b"render_warps", 12)):
+        assert _lib.lib().ia_set_option(name, ctypes.c_int(value)) == -1, name
+        assert b"unknown option" in _lib.lib().ia_last_error(), name
+    # retired values of the remaining options are refused
+    for name, value in ((b"render_rays_per_warp", 8), (b"render_rays_per_warp", 16), (b"render_rays_per_warp", 32),
+                        (b"query_warps", 20)):
+        assert _lib.lib().ia_set_option(name, ctypes.c_int(value)) == -1, (name, value)
+        assert b"invalid argument" in _lib.lib().ia_last_error(), (name, value)
     # every option bench.py reports is readable
     bench = open(os.path.join(os.path.dirname(os.path.dirname(os.path.abspath(__file__))), "bench.py")).read()
     names = set(re.findall(r"""get_option\(\s*["'](\w+)["']""", bench))
