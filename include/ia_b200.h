@@ -536,6 +536,49 @@ size_t ia_gif_quantize_workspace_bytes(int F);
 int ia_gif_quantize(const uint8_t* rgba, int F, int H, int W, int swap_rb, uint8_t* palette, uint8_t* index, int* n_colors,
                     void* workspace, size_t workspace_bytes, ia_stream_t stream);
 
+/* Batched SMPL forward and reverse mode for fitting F frames of poses to 2D keypoints: the keypoint stage of
+ * refine-smpl.py (scripts/custom/refine-smpl.py:166-189; DESIGN.md §3, §5.10).  fp32 throughout.
+ *
+ * Model (device, fp32, the layouts of instantavatar_b200.deformers.smpl.SMPL): v_template [V][3], shapedirs [V][3][10],
+ * posedirs [207][3V], J_regressor [24][V] (dense), lbs_weights [V][24], parents [24] int32 (-1 for the root).
+ * params: one flat vector [10 + 75F] = betas [10] | global_orient [F][3] | body_pose [F][69] | transl [F][3]; betas are
+ * shared by every frame.  workspace: device, 16-byte aligned, ia_smpl_fit_workspace_bytes(V, F) bytes (0 for invalid
+ * sizes).  No host synchronisation; two calls on the same input give bit-identical results (fixed-order reductions).
+ *
+ * ia_smpl_fit_forward: verts [F][V][3], joints [F][35][3] (the 24 posed joints, then the vertices vertex_ids [11], host),
+ *   A [F][24][4][4] (the bone transforms with transl, as smplx returns them); each output nullable.
+ * ia_smpl_fit_objective: loss [1] (device, nullable) and grad [10 + 75F] (written, in the layout of params) of
+ *     mean_{f, b selected} m_fb |kp_fb - uv_fb|  +  mean_{f < F-1, v} |verts[f+1][v] - verts[f][v]|
+ *   where BODY25 joint b is smplx joint joint_map[b] (0..23 posed joint, 24 + k vertex joint k), uv is its projection by
+ *   proj = K . E[:3] (host, [3][4] row-major): uv = p[:2] / p[2], p = proj[:, :3] x + proj[:, 3]; m_fb = conf_fb > threshold;
+ *   the first mean is over F * (number of selected b), masked entries included.  A residual of exactly zero contributes a
+ *   zero gradient.  keypoints [F][25][3] (device; u, v, confidence).  IA_EINVAL: F < 2, no selected joint, a joint_map
+ *   entry outside [0, 35), a vertex id outside [0, V). */
+typedef struct {
+    const float* v_template;
+    const float* shapedirs;
+    const float* posedirs;
+    const float* J_regressor;
+    const float* lbs_weights;
+    const int* parents;
+    int n_verts;
+} IaSmplModel;
+
+typedef struct {
+    const float* keypoints;   /* device [F][25][3] */
+    const float* proj;        /* host [3][4] */
+    const int* joint_map;     /* host [25] */
+    const int* select;        /* host [25], non-zero: in the keypoint mean */
+    const int* vertex_ids;    /* host [11] */
+    float threshold;
+} IaKeypointFit;
+
+size_t ia_smpl_fit_workspace_bytes(int n_verts, int F);
+int ia_smpl_fit_forward(const IaSmplModel* model /*[host]*/, const float* params, int F, const int* vertex_ids /*[host]*/,
+                        void* workspace, size_t workspace_bytes, float* verts, float* joints, float* A, ia_stream_t stream);
+int ia_smpl_fit_objective(const IaSmplModel* model /*[host]*/, const IaKeypointFit* fit /*[host]*/, const float* params, int F,
+                          void* workspace, size_t workspace_bytes, float* loss, float* grad, ia_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -31,7 +31,18 @@ SYMBOLS = [
     "ia_mc_workspace_bytes", "ia_mc_count", "ia_mc_emit", "ia_mc_component_workspace_bytes", "ia_mc_largest_component",
     "ia_skin_points", "ia_frame_index_bytes", "ia_frame_index_build", "ia_sample_edge", "ia_sample_patch",
     "ia_test_panel", "ia_image_metrics", "ia_gif_quantize_workspace_bytes", "ia_gif_quantize",
+    "ia_smpl_fit_workspace_bytes", "ia_smpl_fit_forward", "ia_smpl_fit_objective",
 ]
+
+
+class IaSmplModel(C.Structure):
+    _fields_ = [("v_template", C.c_void_p), ("shapedirs", C.c_void_p), ("posedirs", C.c_void_p), ("J_regressor", C.c_void_p),
+                ("lbs_weights", C.c_void_p), ("parents", C.c_void_p), ("n_verts", C.c_int32)]
+
+
+class IaKeypointFit(C.Structure):
+    _fields_ = [("keypoints", C.c_void_p), ("proj", C.c_void_p), ("joint_map", C.c_void_p), ("select", C.c_void_p),
+                ("vertex_ids", C.c_void_p), ("threshold", C.c_float)]
 
 
 class IaNearestVertex(C.Structure):
@@ -81,6 +92,7 @@ def lib():
         _lib.ia_mc_component_workspace_bytes.restype = C.c_size_t
         _lib.ia_frame_index_bytes.restype = C.c_size_t
         _lib.ia_gif_quantize_workspace_bytes.restype = C.c_size_t
+        _lib.ia_smpl_fit_workspace_bytes.restype = C.c_size_t
         for s in SYMBOLS:
             getattr(_lib, s)  # fail loudly on a stale library
         if _lib.ia_abi_version() != 1:

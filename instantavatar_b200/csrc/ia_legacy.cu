@@ -7,6 +7,7 @@
 #include <stdint.h>
 
 #include "ia_host.h"
+#include "ia_smpl.cuh"
 
 namespace {
 
@@ -149,52 +150,18 @@ int ia_composite_test(const float* rgb_vals, const float* sigma_vals, const floa
 //   w2s   = A_0^-1 (rigid, closed form) ;  tfs_j = w2s . A_j . tfs_inv_t_j
 namespace {
 
-__device__ __forceinline__ void mat4_mul(const float* a, const float* b, float* c) {
-    for (int i = 0; i < 4; i++)
-        for (int j = 0; j < 4; j++) {
-            float s = 0.f;
-            for (int k = 0; k < 4; k++) s = __fmaf_rn(a[i * 4 + k], b[k * 4 + j], s);
-            c[i * 4 + j] = s;
-        }
-}
-
 __global__ void __launch_bounds__(32) smpl_tfs_kernel(const float* __restrict__ global_orient, const float* __restrict__ body_pose,
                                                       const float* __restrict__ transl, const float* __restrict__ J,
                                                       const int* __restrict__ parents, const float* __restrict__ tfs_inv_t,
                                                       float* __restrict__ tfs, float* __restrict__ w2s_out, float* __restrict__ A_out) {
     __shared__ float tm[24][16], chain[24][16], A[24][16], w2s[16];
     const int j = threadIdx.x;
-    if (j < 24) {
-        // Rodrigues (lbs.py:295-329): angle = ||r + 1e-8||, K from r/angle, R = I + sin K + (1-cos) K^2
-        const float* r = j == 0 ? global_orient : body_pose + (j - 1) * 3;
-        const float ax = r[0] + 1e-8f, ay = r[1] + 1e-8f, az = r[2] + 1e-8f;
-        const float angle = sqrtf(ax * ax + ay * ay + az * az);
-        const float rx = r[0] / angle, ry = r[1] / angle, rz = r[2] / angle;
-        const float s = sinf(angle), c = 1.f - cosf(angle);
-        const float K[9] = {0.f, -rz, ry, rz, 0.f, -rx, -ry, rx, 0.f};
-        float K2[9];
-        for (int a = 0; a < 3; a++)
-            for (int b = 0; b < 3; b++) K2[a * 3 + b] = K[a * 3] * K[b] + K[a * 3 + 1] * K[3 + b] + K[a * 3 + 2] * K[6 + b];
-        const int p = parents[j];
-        for (int a = 0; a < 3; a++) {
-            for (int b = 0; b < 3; b++) tm[j][a * 4 + b] = (a == b ? 1.f : 0.f) + s * K[a * 3 + b] + c * K2[a * 3 + b];
-            tm[j][a * 4 + 3] = J[j * 3 + a] - (j > 0 ? J[p * 3 + a] : 0.f);
-        }
-        tm[j][12] = tm[j][13] = tm[j][14] = 0.f; tm[j][15] = 1.f;
-    }
+    if (j < 24) smpl_local_transform(j, j == 0 ? global_orient : body_pose + (j - 1) * 3, J, parents, tm[j]);
     __syncwarp();
-    if (j == 0) {  // kinematic chain (24 tiny products; sequential dependency along the tree)
-        for (int e = 0; e < 16; e++) chain[0][e] = tm[0][e];
-        for (int i = 1; i < 24; i++) mat4_mul(chain[parents[i]], tm[i], chain[i]);
-    }
+    if (j == 0) smpl_chain(parents, tm, chain);
     __syncwarp();
     if (j < 24) {
-        // A = chain - pad(chain . [J;0])  (lbs.py:396-399), then + transl
-        for (int e = 0; e < 16; e++) A[j][e] = chain[j][e];
-        for (int a = 0; a < 3; a++) {
-            const float tj = chain[j][a * 4] * J[j * 3] + chain[j][a * 4 + 1] * J[j * 3 + 1] + chain[j][a * 4 + 2] * J[j * 3 + 2];
-            A[j][a * 4 + 3] = chain[j][a * 4 + 3] - tj + (transl ? transl[a] : 0.f);
-        }
+        smpl_rest_relative(j, chain[j], J, transl, A[j]);
         if (A_out) for (int e = 0; e < 16; e++) A_out[j * 16 + e] = A[j][e];
     }
     __syncwarp();
@@ -209,8 +176,8 @@ __global__ void __launch_bounds__(32) smpl_tfs_kernel(const float* __restrict__ 
     __syncwarp();
     if (j < 24) {
         float t1[16], t2[16];
-        mat4_mul(w2s, A[j], t1);
-        mat4_mul(t1, tfs_inv_t + j * 16, t2);
+        smpl_mat4_mul(w2s, A[j], t1);
+        smpl_mat4_mul(t1, tfs_inv_t + j * 16, t2);
         for (int e = 0; e < 16; e++) tfs[j * 16 + e] = t2[e];
     }
 }
@@ -232,39 +199,13 @@ __global__ void __launch_bounds__(32) smpl_tfs_bwd_kernel(const float* __restric
     __shared__ float tm[24][16], chain[24][16], A[24][16], w2s[16];
     __shared__ float gA[24][12], gC[24][12], gW[12], gL[24][9];
     const int j = threadIdx.x;
-    // ---- forward recomputation (identical expressions to smpl_tfs_kernel) ----
-    float rr[3] = {0.f, 0.f, 0.f}, angle = 1.f;
-    if (j < 24) {
-        const float* r = j == 0 ? global_orient : body_pose + (j - 1) * 3;
-        rr[0] = r[0]; rr[1] = r[1]; rr[2] = r[2];
-        const float ax = r[0] + 1e-8f, ay = r[1] + 1e-8f, az = r[2] + 1e-8f;
-        angle = sqrtf(ax * ax + ay * ay + az * az);
-        const float rx = r[0] / angle, ry = r[1] / angle, rz = r[2] / angle;
-        const float s = sinf(angle), c = 1.f - cosf(angle);
-        const float K[9] = {0.f, -rz, ry, rz, 0.f, -rx, -ry, rx, 0.f};
-        float K2[9];
-        for (int a = 0; a < 3; a++)
-            for (int b = 0; b < 3; b++) K2[a * 3 + b] = K[a * 3] * K[b] + K[a * 3 + 1] * K[3 + b] + K[a * 3 + 2] * K[6 + b];
-        const int p = parents[j];
-        for (int a = 0; a < 3; a++) {
-            for (int b = 0; b < 3; b++) tm[j][a * 4 + b] = (a == b ? 1.f : 0.f) + s * K[a * 3 + b] + c * K2[a * 3 + b];
-            tm[j][a * 4 + 3] = J[j * 3 + a] - (j > 0 ? J[p * 3 + a] : 0.f);
-        }
-        tm[j][12] = tm[j][13] = tm[j][14] = 0.f; tm[j][15] = 1.f;
-    }
+    // ---- forward recomputation (the same device functions as smpl_tfs_kernel) ----
+    const float* r = j == 0 ? global_orient : body_pose + (j - 1) * 3;
+    if (j < 24) smpl_local_transform(j, r, J, parents, tm[j]);
     __syncwarp();
-    if (j == 0) {
-        for (int e = 0; e < 16; e++) chain[0][e] = tm[0][e];
-        for (int i = 1; i < 24; i++) mat4_mul(chain[parents[i]], tm[i], chain[i]);
-    }
+    if (j == 0) smpl_chain(parents, tm, chain);
     __syncwarp();
-    if (j < 24) {
-        for (int e = 0; e < 16; e++) A[j][e] = chain[j][e];
-        for (int a = 0; a < 3; a++) {
-            const float tj = chain[j][a * 4] * J[j * 3] + chain[j][a * 4 + 1] * J[j * 3 + 1] + chain[j][a * 4 + 2] * J[j * 3 + 2];
-            A[j][a * 4 + 3] = chain[j][a * 4 + 3] - tj + (transl ? transl[a] : 0.f);
-        }
-    }
+    if (j < 24) smpl_rest_relative(j, chain[j], J, transl, A[j]);
     __syncwarp();
     if (j == 0) {
         for (int a = 0; a < 3; a++) {
@@ -329,51 +270,11 @@ __global__ void __launch_bounds__(32) smpl_tfs_bwd_kernel(const float* __restric
         if (j == 0 && g_transl) g_transl[a] = transl ? v : 0.f;
     }
     __syncwarp();
-    // ---- chain, children before parents (parents[i] < i): C_i = C_p L_i ----
-    if (j == 0) {
-        for (int i = 23; i >= 1; i--) {
-            const int p = parents[i];
-            const float* Cp = chain[p]; const float* L = tm[i];
-            for (int a = 0; a < 3; a++) {
-                for (int b = 0; b < 3; b++) {
-                    // gL.R = Cp.R^T gC_i.R
-                    gL[i][a * 3 + b] = Cp[a] * gC[i][b] + Cp[4 + a] * gC[i][4 + b] + Cp[8 + a] * gC[i][8 + b];
-                    // gCp.R += gC_i.R L.R^T + gC_i.t L.t^T
-                    gC[p][a * 4 + b] += gC[i][a * 4] * L[b * 4] + gC[i][a * 4 + 1] * L[b * 4 + 1] + gC[i][a * 4 + 2] * L[b * 4 + 2]
-                                        + gC[i][a * 4 + 3] * L[b * 4 + 3];
-                }
-                gC[p][a * 4 + 3] += gC[i][a * 4 + 3];
-            }
-        }
-        for (int a = 0; a < 3; a++)
-            for (int b = 0; b < 3; b++) gL[0][a * 3 + b] = gC[0][a * 4 + b];
-    }
+    if (j == 0) smpl_chain_bwd(parents, tm, chain, gC, gL, nullptr);
     __syncwarp();
-    // ---- Rodrigues: d R / d r_k, contracted with gL ----
     if (j < 24) {
-        const float a3[3] = {rr[0] + 1e-8f, rr[1] + 1e-8f, rr[2] + 1e-8f};
-        const float th = angle, s = sinf(th), c = cosf(th);
-        const float n[3] = {rr[0] / th, rr[1] / th, rr[2] / th};
-        const float K[9] = {0.f, -n[2], n[1], n[2], 0.f, -n[0], -n[1], n[0], 0.f};
-        float K2[9];
-        for (int a = 0; a < 3; a++)
-            for (int b = 0; b < 3; b++) K2[a * 3 + b] = K[a * 3] * K[b] + K[a * 3 + 1] * K[3 + b] + K[a * 3 + 2] * K[6 + b];
         float out[3];
-        for (int k = 0; k < 3; k++) {
-            const float dth = a3[k] / th;
-            float dn[3];
-            for (int d = 0; d < 3; d++) dn[d] = (d == k ? 1.f / th : 0.f) - rr[d] * dth / (th * th);
-            const float dK[9] = {0.f, -dn[2], dn[1], dn[2], 0.f, -dn[0], -dn[1], dn[0], 0.f};
-            float acc = 0.f;
-            for (int a = 0; a < 3; a++)
-                for (int b = 0; b < 3; b++) {
-                    float dKK = 0.f;  // dK K + K dK
-                    for (int m = 0; m < 3; m++) dKK += dK[a * 3 + m] * K[m * 3 + b] + K[a * 3 + m] * dK[m * 3 + b];
-                    const float dR = c * dth * K[a * 3 + b] + s * dK[a * 3 + b] + s * dth * K2[a * 3 + b] + (1.f - c) * dKK;
-                    acc += gL[j][a * 3 + b] * dR;
-                }
-            out[k] = acc;
-        }
+        smpl_rodrigues_bwd(r, gL[j], out);
         float* dst = j == 0 ? g_orient : g_pose + (j - 1) * 3;
         if (dst) { dst[0] = out[0]; dst[1] = out[1]; dst[2] = out[2]; }
     }

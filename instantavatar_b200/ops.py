@@ -809,6 +809,81 @@ def gif_quantize(rgba, swap_rb: bool = False):
     return palette, index, n_colors
 
 
+@dataclass
+class SmplFitModel:
+    """Device tables of an SMPL body model for the batched fitting kernels (IaSmplModel): the buffers of
+    deformers.smpl.SMPL in fp32 and its parents as int32."""
+    v_template: torch.Tensor
+    shapedirs: torch.Tensor
+    posedirs: torch.Tensor
+    J_regressor: torch.Tensor
+    lbs_weights: torch.Tensor
+    parents: torch.Tensor
+
+    @classmethod
+    def from_smpl(cls, smpl, device):
+        g = lambda t: t.detach().to(device=device, dtype=f32).contiguous()
+        return cls(g(smpl.v_template), g(smpl.shapedirs), g(smpl.posedirs), g(smpl.J_regressor), g(smpl.lbs_weights),
+                   smpl.parents.to(device=device, dtype=torch.int32).contiguous())
+
+    @property
+    def n_verts(self) -> int:
+        return self.v_template.shape[0]
+
+    def c_struct(self) -> _lib.IaSmplModel:
+        s = _lib.IaSmplModel()
+        s.v_template = ptr(self.v_template, f32).value; s.shapedirs = ptr(self.shapedirs, f32).value
+        s.posedirs = ptr(self.posedirs, f32).value; s.J_regressor = ptr(self.J_regressor, f32).value
+        s.lbs_weights = ptr(self.lbs_weights, f32).value; s.parents = ptr(self.parents, torch.int32).value
+        s.n_verts = self.n_verts
+        return s
+
+
+def smpl_fit_workspace(model: SmplFitModel, F: int) -> torch.Tensor:
+    nbytes = int(lib().ia_smpl_fit_workspace_bytes(C.c_int(model.n_verts), C.c_int(F)))
+    if nbytes == 0:
+        raise ValueError(f"smpl_fit: invalid sizes V={model.n_verts} F={F}")
+    return torch.empty(nbytes, device=model.v_template.device, dtype=torch.uint8)
+
+
+def _int_array(values, n: int, name: str):
+    values = [int(v) for v in values]
+    if len(values) != n:
+        raise ValueError(f"{name} must have {n} entries, got {len(values)}")
+    return (C.c_int * n)(*values)
+
+
+def smpl_fit_forward(model: SmplFitModel, params, F: int, vertex_ids, workspace=None):
+    """Batched SMPL forward of the flat parameters [10 + 75F] (betas | global_orient | body_pose | transl) ->
+    (verts [F,V,3], joints [F,35,3] = 24 posed joints + the 11 vertex joints vertex_ids, A [F,24,4,4] with transl)."""
+    dev = params.device
+    workspace = smpl_fit_workspace(model, F) if workspace is None else workspace
+    verts = torch.empty((F, model.n_verts, 3), device=dev, dtype=f32)
+    joints = torch.empty((F, 35, 3), device=dev, dtype=f32)
+    A = torch.empty((F, 24, 4, 4), device=dev, dtype=f32)
+    s = model.c_struct()
+    _lib.count(6); check(lib().ia_smpl_fit_forward(C.byref(s), ptr(params, f32), C.c_int(F), _int_array(vertex_ids, 11, "vertex_ids"),
+                                                   ptr(workspace), C.c_size_t(workspace.numel()), ptr(verts), ptr(joints), ptr(A), stream()))
+    return verts, joints, A
+
+
+def smpl_fit_objective(model: SmplFitModel, params, F: int, keypoints, proj, joint_map, select, vertex_ids, threshold: float,
+                       workspace, grad, loss=None):
+    """Keypoint objective of refine-smpl.py and its gradient in the layout of params, in 13 launches without host reads:
+    keypoints [F,25,3] (device), proj [3,4] (host), joint_map / select [25] and vertex_ids [11] (host).  loss: device
+    scalar (nullable); grad: [10 + 75F], written."""
+    s = model.c_struct()
+    fit = _lib.IaKeypointFit()
+    P = (C.c_float * 12)(*[float(x) for x in torch.as_tensor(proj, dtype=torch.float64).reshape(-1).tolist()])
+    jm, sel, vid = _int_array(joint_map, 25, "joint_map"), _int_array(select, 25, "select"), _int_array(vertex_ids, 11, "vertex_ids")
+    fit.keypoints = ptr(keypoints, f32).value
+    fit.proj = C.cast(P, C.c_void_p).value; fit.joint_map = C.cast(jm, C.c_void_p).value
+    fit.select = C.cast(sel, C.c_void_p).value; fit.vertex_ids = C.cast(vid, C.c_void_p).value
+    fit.threshold = float(threshold)
+    _lib.count(13); check(lib().ia_smpl_fit_objective(C.byref(s), C.byref(fit), ptr(params, f32), C.c_int(F), ptr(workspace),
+                                                      C.c_size_t(workspace.numel()), ptr(loss, f32), ptr(grad, f32), stream()))
+
+
 # ------------------------------------------------------------------------------------------------------------------
 # device guard: every operator launches on the current stream OF THE DEVICE ITS TENSORS LIVE ON (one process may hold
 # tensors on several GPUs; function attributes and SM counts are cached per device inside the library)
