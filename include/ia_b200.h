@@ -83,8 +83,8 @@ const char* ia_last_error(void);
 int ia_sm_count(void);
 
 /* tuning knobs (do not change results): "render_rays_per_warp" in {4, 2, 1} (ray tile of ia_render_fwd*; the sharded
- * frame uses 2 and 1), "query_warps" in {12, 16} (warps per CTA of ia_occupancy_query* and of ia_deform_query without
- * xc_best, Fast-SNARF scenes), "query_lanes_per_sample" in {0 = from the load, 1, 2, 4} (lanes sharing one sample's 13 root finds in
+ * frame uses 2 and 1), "query_warps" in {12, 16} (warps per CTA of ia_deform_query without xc_best, Fast-SNARF scenes),
+ * "query_lanes_per_sample" in {0 = from the load, 1, 2, 4} (lanes sharing one sample's 13 root finds in
  * ia_train_fwd_split's point query).  Any other name is IA_EINVAL ("unknown option"). */
 int ia_set_option(const char* name, int value);
 
@@ -232,13 +232,17 @@ int ia_render_fwd_peer(const IaScene* scene /*[host]*/, const float* rays_o, con
 int ia_deform_query(const IaScene* scene /*[host]*/, const float* pts, int n, int eval_mode, float* rgb, float* sigma,
                     float* xc_best, int8_t* best_init, IaStats* stats, ia_stream_t stream);
 
-/* DensityGrid.initialize's density pass (models/structures/density_grid.py:94-103) in one launch: for each of
- * `passes` jitter tensors [G][G][G][3] the G^3 cell points (idx/G + jitter/G) * (max - min) + min are queried in eval
- * mode and max(sigma, 0) is reduced into density_max [G][G][G] (zeroed by the library).  aabb [6] device.
- * workspace: nullable; >= 256 bytes enables dynamic batch scheduling.  shard / n_shards: this call evaluates every
- * n_shards-th batch of cells starting at `shard` (multi-GPU: the caller max-all-reduces density_max; 0 / 1 = all). */
+/* DensityGrid.initialize's density pass (models/structures/density_grid.py:94-103): for each of `passes` jitter tensors
+ * [G][G][G][3] the G^3 cell points (idx/G + jitter/G) * (max - min) + min are queried in eval mode and max(sigma, 0) is
+ * reduced into density_max [G][G][G] (zeroed by the library).  aabb [6] device.  Two launches: root finding appends every
+ * kept root to a list in `workspace`, then the network evaluates the list.  workspace: device, at least
+ * ia_occupancy_query_workspace_bytes(G, passes, n_shards) bytes.  shard / n_shards: this call evaluates every n_shards-th
+ * batch of cells starting at `shard` (multi-GPU: the caller max-all-reduces density_max; 0 / 1 = all). */
 int ia_occupancy_query(const IaScene* scene /*[host]*/, const float* jitter, const float* aabb, int G, int passes,
                        float* density_max, void* workspace, int shard, int n_shards, IaStats* stats, ia_stream_t stream);
+/* bytes of ia_occupancy_query*'s workspace: counters, root-finding scratch and a root list that holds the shard's worst
+ * case (all 13 roots of every grid point kept; 272 MB at G = 64, 5 passes, 1 shard); 0 for invalid arguments [host] */
+size_t ia_occupancy_query_workspace_bytes(int G, int passes, int n_shards);
 
 /* ia_occupancy_query over peer memory: this rank's shard of the cells is max-reduced into the density grid of EVERY rank
  * with NVLink atomics (positive densities only: ~2 % of the cells), replacing the 1 MB max-all-reduce.  peer_density: DEVICE

@@ -22,7 +22,7 @@ IA_MAX_SAMPLES = 256
 
 SYMBOLS = [
     "ia_abi_version", "ia_last_error", "ia_sm_count", "ia_set_option", "ia_hashgrid_layout", "ia_precompute", "ia_params_to_half",
-    "ia_pack_occupancy", "ia_occupancy_build", "ia_render_workspace_bytes", "ia_occupancy_query", "ia_composite_bwd", "ia_ngp_backward",
+    "ia_pack_occupancy", "ia_occupancy_build", "ia_render_workspace_bytes", "ia_occupancy_query", "ia_occupancy_query_workspace_bytes", "ia_composite_bwd", "ia_ngp_backward",
     "ia_ngp_backward_scratch_bytes", "ia_adam_step", "ia_grad_check_finite", "ia_adam_prepare", "ia_adam_step_dev",
     "ia_mlp_to_half", "ia_raymarch_train", "ia_raymarch_test", "ia_composite_test", "ia_smpl_tfs", "ia_nerf_loss", "ia_pose_grad", "ia_knn1", "ia_smpl_tfs_backward", "ia_ngp_input_grad", "ia_voxelize_weights", "ia_render_fwd", "ia_deform_query", "ia_broyden", "ia_ngp_forward", "ia_transform_rays", "ia_mlp_to_half_from_half", "ia_grad_poison_shards", "ia_gather_ceiling", "ia_tcnn_backward_scratch_bytes", "ia_tcnn_encoder_forward",
     "ia_tcnn_encoder_backward", "ia_tcnn_mlp_forward", "ia_tcnn_mlp_backward", "ia_render_fwd_peer", "ia_occupancy_query_peer", "ia_peer_reduce_check",
@@ -85,6 +85,7 @@ def lib():
         _lib.ia_last_error.restype = C.c_char_p
         _lib.ia_ngp_backward_scratch_bytes.restype = C.c_size_t
         _lib.ia_render_workspace_bytes.restype = C.c_size_t
+        _lib.ia_occupancy_query_workspace_bytes.restype = C.c_size_t
         _lib.ia_tcnn_backward_scratch_bytes.restype = C.c_size_t
         _lib.ia_train_fwd_workspace_bytes.restype = C.c_size_t
         _lib.ia_nv_workspace_bytes.restype = C.c_size_t

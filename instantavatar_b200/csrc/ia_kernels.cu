@@ -386,20 +386,15 @@ __global__ void __launch_bounds__(kRenderWarps * 32, 1) render_fwd_kernel(const 
 }
 
 // ================================================================================================
-// point query (DensityGrid passes, legacy model(pts) path)
+// point query (DensityGrid.update, legacy model(pts) path, split training forward)
 // ================================================================================================
 struct QueryArgs {
     SceneDev sd;
     const float* pts; int n; int eval_mode;
     float* rgb; float* sigma; float* xc_best; int8_t* best_init;
     IaStats* stats;
-    // grid mode (DensityGrid.initialize, density_grid.py:94-103): points are generated from the cell index and the
-    // per-pass jitter, and max(sigma, 0) is reduced over the passes into density_max[G^3]
-    const float* grid_jitter; const float* grid_aabb; int G; float* density_max; int passes;
     int* batch_counter;  // optional: dynamic batch scheduling (zeroed by the launcher)
-    int batch_first, batch_stride;  // grid mode: this launch handles batches first, first+stride, ... (multi-GPU sharding)
-    float* const* peer_density; int n_peers;  // grid mode over peer memory: max-reduce into EVERY rank's density (NVLink atomics)
-    // point mode, optional (split training forward, ia_train.cu): the number of points lives on the device (n = capacity)
+    // optional (split training forward, ia_train.cu): the number of points lives on the device (n = capacity)
     // and point p reads pts / writes every output at element index[p] instead of p
     const int* n_dev; const int* index;
     int lanes_per_sample;  // point mode: 1 / 2 / 4 lanes share a point's 13 root finds (narrow batches); 0 = pick from the load
@@ -413,9 +408,9 @@ struct QuerySmem {
     std::conditional_t<kNV, WarpScratchNV, WarpScratch<kKeepXc>> ws[kWarps];
 };
 
-// kKeepXc: the canonical point of the winning candidate is an output (xc_best; training-time queries); the occupancy
-// passes do not need it, which frees 5 KB of shared memory per warp.  Fast-SNARF queries that keep it choose the lanes
-// per point at run time (a.lanes_per_sample); the occupancy passes run one lane per point with a literal 1
+// kKeepXc: the canonical point of the winning candidate is an output (xc_best; training-time queries); queries without
+// it need 5 KB less shared memory per warp.  Fast-SNARF queries that keep it choose the lanes per point at run time
+// (a.lanes_per_sample); the others run one lane per point with a literal 1
 // kNV: nearest-vertex deform stage (warp_eval_nv, one lane per point)
 template <int kWarps, bool kKeepXc, bool kNV = false>
 __global__ void __launch_bounds__(kWarps * 32, 1) deform_query_kernel(const __grid_constant__ QueryArgs a) {
@@ -436,9 +431,6 @@ __global__ void __launch_bounds__(kWarps * 32, 1) deform_query_kernel(const __gr
     ctx.table = reinterpret_cast<const __half2*>(a.sd.s.table_h);
     ctx.Wsm = sm.W; ctx.fc = &sm.fc; ctx.hl = &a.sd.hl;
     unsigned st_gather = 0, st_roots = 0, st_samples = 0, st_load = 0, st_hash = 0;
-    // grid mode: a batch holds all jitter passes of 32/passes neighbouring cells, so that the 32 lanes stay within a
-    // few voxels of the skinning field (L1 wavefronts, not DRAM, bound this kernel)
-    const int n3g = a.G * a.G * a.G;
     const int n_pts = a.n_dev ? min(*a.n_dev, a.n) : a.n;
     // with few points per resident warp a batch's latency (13 serial root finds per lane) is the kernel's time; k lanes per
     // point divide it (warp_eval_samples) at no extra memory traffic.  Point mode, k = 0: about one batch per warp.
@@ -451,44 +443,21 @@ __global__ void __launch_bounds__(kWarps * 32, 1) deform_query_kernel(const __gr
         }
     }
     const int spw = 32 / k;  // points per warp batch
-    const int cells_per_batch = a.grid_aabb ? spw / a.passes : spw;
-    const int n_batches = a.grid_aabb ? (n3g + cells_per_batch - 1) / cells_per_batch : (n_pts + spw - 1) / spw;
-    for (int lidx = blockIdx.x * kWarps + warp;; lidx += gridDim.x * kWarps) {
+    const int n_batches = (n_pts + spw - 1) / spw;
+    for (int bidx = blockIdx.x * kWarps + warp;; bidx += gridDim.x * kWarps) {
         if (a.batch_counter) {  // dynamic: batches near the body cost several times more than empty space
             int nb = 0;
             if (lane == 0) nb = atomicAdd(a.batch_counter, 1);
-            lidx = __shfl_sync(kFull, nb, 0);
+            bidx = __shfl_sync(kFull, nb, 0);
         }
-        const int bidx = a.batch_first + lidx * a.batch_stride;
-        if (bidx >= n_batches || bidx < 0) break;
-        int p = bidx * spw + (lane & (spw - 1));
+        if (bidx >= n_batches) break;
+        const int p = bidx * spw + (lane & (spw - 1));
         bool act = p < n_pts;
         const bool owner = lane < spw;  // helper lanes (k > 1) evaluate some of their point's root finds, nothing else
         long q = p;  // element the point is read from / written to
         if (act && a.index) q = a.index[p];
         float x = 0, y = 0, z = 0;
-        int cell = 0;
-        if (a.grid_aabb) {
-            const int pl = lane & (spw - 1);  // point slot inside the batch (helper lanes repeat their owner's)
-            cell = bidx * cells_per_batch + pl / a.passes;
-            const int pass = pl % a.passes;
-            act = pl < cells_per_batch * a.passes && cell < n3g;
-            p = pass * n3g + cell;
-        }
-        if (act) {
-            if (a.grid_aabb) {
-                // coords = (idx / G + jitter / G) * (max - min) + min   (density_grid.py:20-23,100)
-                const int G = a.G;
-                const int ci = cell / (G * G), cj = (cell / G) % G, ck = cell % G;
-                const float* jit = a.grid_jitter + (long)p * 3;
-                const float fG = (float)G;
-                x = ((float)ci / fG + jit[0] / fG) * (a.grid_aabb[3] - a.grid_aabb[0]) + a.grid_aabb[0];
-                y = ((float)cj / fG + jit[1] / fG) * (a.grid_aabb[4] - a.grid_aabb[1]) + a.grid_aabb[1];
-                z = ((float)ck / fG + jit[2] / fG) * (a.grid_aabb[5] - a.grid_aabb[2]) + a.grid_aabb[2];
-            } else {
-                x = a.pts[q * 3]; y = a.pts[q * 3 + 1]; z = a.pts[q * 3 + 2];
-            }
-        }
+        if (act) { x = a.pts[q * 3]; y = a.pts[q * 3 + 1]; z = a.pts[q * 3 + 2]; }
         SampleOut so;
         if constexpr (kNV) {
             warp_eval_nv(ctx, a.sd.nv, sm.ws[warp], act, x, y, z, a.eval_mode != 0, lane, so, st_roots, st_hash);
@@ -499,17 +468,7 @@ __global__ void __launch_bounds__(kWarps * 32, 1) deform_query_kernel(const __gr
         }
         act = act && owner;
         st_samples += act ? 1u : 0u;
-        if (act && a.grid_aabb) {
-            if (so.sigma > 0.f) {
-                // positive densities are ~2 % of the cells: with peer pointers the cross-GPU max-reduction is these few
-                // atomics over NVLink instead of a 1 MB all-reduce after the kernel
-                if (a.peer_density) {
-                    for (int pr = 0; pr < a.n_peers; pr++) atomicMax(reinterpret_cast<int*>(a.peer_density[pr]) + cell, __float_as_int(so.sigma));
-                } else {
-                    atomicMax(reinterpret_cast<int*>(a.density_max) + cell, __float_as_int(so.sigma));
-                }
-            }
-        } else if (act) {
+        if (act) {
             a.sigma[q] = so.sigma;
             a.rgb[q * 3] = so.r; a.rgb[q * 3 + 1] = so.g; a.rgb[q * 3 + 2] = so.b;
             if constexpr (kKeepXc) {
@@ -534,6 +493,194 @@ __global__ void __launch_bounds__(kWarps * 32, 1) deform_query_kernel(const __gr
             atomicAdd(&a.stats->net_evals, (unsigned long long)st_roots);
             atomicAdd(&a.stats->samples, (unsigned long long)st_samples);
         }
+    }
+}
+
+// ================================================================================================
+// occupancy pass (DensityGrid.initialize, density_grid.py:94-103) in two launches: root finding -> root list -> network.
+// The root finding is a chain of serial, data-dependent field gathers per lane; the network needs the weights, the
+// feature tiles and the MMA fragments.  Apart, each runs at the residency that suits it (DESIGN §5.2).
+// ================================================================================================
+struct OccRoot { float x, y, z; int cell; };  // canonical root of a kept candidate and the cell of its grid point
+
+struct OccArgs {
+    SceneDev sd;
+    const float* grid_jitter; const float* grid_aabb; int G, passes;
+    int* counters;  // [0] batch counter (dynamic scheduling), [1] number of roots in `roots`; zeroed by the launcher
+    float* cand;  // root finding's per-warp candidate scratch [warp][3][kNumInit][32]
+    OccRoot* roots;  // worst case: kNumInit roots per grid point of this shard
+    int batch_first, batch_stride;  // this launch handles batches first, first+stride, ... (multi-GPU sharding)
+    float* density_max;
+    float* const* peer_density; int n_peers;  // max-reduce into EVERY rank's density (NVLink atomics) instead
+    IaStats* stats;
+};
+
+// Root finding runs 16 warps per SM at 128 registers; its candidates live in global scratch, not shared memory, so that
+// nearly all of the SM's 256 KB of L1 / shared memory serves the field gathers as L1 (DESIGN §5.2)
+constexpr int kOccRootWarps = 8;      // warps per CTA ...
+constexpr int kOccRootCtas = 2;       // ... and CTAs per SM
+constexpr int kOccRootMaxCtas = 320;  // bound of the grid, and so of the candidate scratch in the workspace
+constexpr int kOccNetWarps = 8;       // network: warps per CTA ...
+constexpr int kOccNetCtas = 4;        // ... and CTAs per SM
+
+// workspace: 256 bytes of counters, the candidate scratch of every root-finding warp, then the root list
+constexpr size_t kOccCandBytes = 256 + sizeof(float) * 3 * kNumInit * 32 * kOccRootWarps * kOccRootMaxCtas;
+
+// a batch holds all jitter passes of 32/passes neighbouring cells, so that the 32 lanes stay within a few voxels of the
+// skinning field (L1 wavefronts, not DRAM, bound the gathers)
+__host__ __device__ inline int occ_cells_per_batch(int passes) { return 32 / passes; }
+__host__ __device__ inline int occ_batches(int G, int passes) {
+    return (G * G * G + occ_cells_per_batch(passes) - 1) / occ_cells_per_batch(passes);
+}
+
+// Kernel A: grid points (density_grid.py:20-23,100) -> 13 Broyden solves + duplicate filter per lane (Fast-SNARF), or the
+// nearest-vertex map -> the kept roots appended to the root list with one atomic per warp
+template <bool kNV>
+__global__ void __launch_bounds__(kOccRootWarps * 32, kOccRootCtas) occupancy_roots_kernel(const __grid_constant__ OccArgs a) {
+    static_assert(kOccRootWarps * 32 >= kNumInit * 12, "load_frame_const stages the bone transforms one thread per entry");
+    __shared__ FrameConst fc;
+    load_frame_const<kNV>(fc, a.sd);
+    __syncthreads();
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    FieldDesc field;
+    field.data = a.sd.s.field; field.D = a.sd.s.D; field.H = a.sd.s.H; field.W = a.sd.s.W;
+    unsigned st_gather = 0, st_roots = 0, st_samples = 0, st_load = 0;
+    // the grid is persistent, so a warp's slot is its own for the whole launch
+    float (*cand)[kNumInit][32] =
+        reinterpret_cast<float (*)[kNumInit][32]>(a.cand + (size_t)(blockIdx.x * kOccRootWarps + warp) * 3 * kNumInit * 32);
+    const int G = a.G, n3g = G * G * G;
+    const int cells_per_batch = occ_cells_per_batch(a.passes);
+    const int n_batches = occ_batches(G, a.passes);
+    for (;;) {
+        int lidx = 0;
+        if (lane == 0) lidx = atomicAdd(&a.counters[0], 1);  // dynamic: batches near the body cost several times more
+        lidx = __shfl_sync(kFull, lidx, 0);
+        const int bidx = a.batch_first + lidx * a.batch_stride;
+        if (bidx >= n_batches) break;
+        const int cell = bidx * cells_per_batch + lane / a.passes;
+        const int pass = lane % a.passes;
+        const bool act = lane < cells_per_batch * a.passes && cell < n3g;
+        float x = 0, y = 0, z = 0;
+        if (act) {
+            // coords = (idx / G + jitter / G) * (max - min) + min   (density_grid.py:20-23,100)
+            const int ci = cell / (G * G), cj = (cell / G) % G, ck = cell % G;
+            const float* jit = a.grid_jitter + ((long)pass * n3g + cell) * 3;
+            const float fG = (float)G;
+            x = ((float)ci / fG + jit[0] / fG) * (a.grid_aabb[3] - a.grid_aabb[0]) + a.grid_aabb[0];
+            y = ((float)cj / fG + jit[1] / fG) * (a.grid_aabb[4] - a.grid_aabb[1]) + a.grid_aabb[1];
+            z = ((float)ck / fG + jit[2] / fG) * (a.grid_aabb[5] - a.grid_aabb[2]) + a.grid_aabb[2];
+        }
+        st_samples += act ? 1u : 0u;
+        unsigned kept = 0;
+        float xc[3] = {0.f, 0.f, 0.f};
+        if constexpr (kNV) {
+            if (act) {
+                float d2;
+                const int v = nv_nearest(a.sd.nv, x, y, z, d2);
+                if (v >= 0) { nv_apply(a.sd.nv, v, x, y, z, xc); kept = 1u; }
+            }
+        } else {
+            kept = warp_find_roots<false>(field, fc, cand, act, x, y, z, lane, st_gather, st_load);
+        }
+        int total;
+        int pos = warp_excl_scan(__popc(kept), lane, total);
+        int base = 0;
+        if (lane == 0 && total) base = atomicAdd(&a.counters[1], total);
+        pos += __shfl_sync(kFull, base, 0);
+        st_roots += __popc(kept);
+        for (unsigned m = kept; m; m &= m - 1) {
+            const int b = __ffs(m) - 1;
+            OccRoot r;
+            if constexpr (kNV) { r.x = xc[0]; r.y = xc[1]; r.z = xc[2]; }
+            else { r.x = cand[0][b][lane]; r.y = cand[1][b][lane]; r.z = cand[2][b][lane]; }
+            r.cell = cell;
+            a.roots[pos++] = r;
+        }
+        __syncwarp();
+    }
+    if (a.stats) {
+#pragma unroll
+        for (int o = 16; o; o >>= 1) {
+            st_gather += __shfl_xor_sync(kFull, st_gather, o);
+            st_load += __shfl_xor_sync(kFull, st_load, o);
+            st_roots += __shfl_xor_sync(kFull, st_roots, o);
+            st_samples += __shfl_xor_sync(kFull, st_samples, o);
+        }
+        if (lane == 0) {
+            atomicAdd(&a.stats->gathers, (unsigned long long)st_gather);
+            atomicAdd(&a.stats->field_loads, (unsigned long long)st_load);
+            atomicAdd(&a.stats->net_evals, (unsigned long long)st_roots);
+            atomicAdd(&a.stats->samples, (unsigned long long)st_samples);
+        }
+    }
+}
+
+// Kernel B: 32 roots per warp -> hash encoding -> density net (mlp_density_tile16, the first half of mlp_tile16: the same
+// sigma bits) -> eval-mode nan_to_num (Fast-SNARF; the nearest-vertex deformer passes its outputs through) -> max into the
+// root's cell.  A cell's value is the max over its passes of max(0, max over kept roots of sigma): max is order-free, so
+// the grid is the fused per-point evaluation's bit for bit.
+template <bool kNanToNum>
+__global__ void __launch_bounds__(kOccNetWarps * 32, kOccNetCtas) occupancy_net_kernel(const __grid_constant__ OccArgs a) {
+    __shared__ __align__(16) __half W[kW3Off];  // density-net block of the padded weights
+    __shared__ __align__(16) __half At[kOccNetWarps][32][kW1Stride];
+    __shared__ float cs[6];
+    const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+    for (int i = threadIdx.x; i < kW3Off / 2; i += blockDim.x)
+        reinterpret_cast<uint32_t*>(W)[i] = reinterpret_cast<const uint32_t*>(a.sd.s.mlp_h)[i];
+    if (threadIdx.x < 3) { cs[threadIdx.x] = a.sd.s.net_center[threadIdx.x]; cs[3 + threadIdx.x] = a.sd.s.net_scale[threadIdx.x]; }
+    __syncthreads();
+    const __half2* table = reinterpret_cast<const __half2*>(a.sd.s.table_h);
+    const int n = a.counters[1];
+    const int g = lane >> 2, t = lane & 3;
+    unsigned st_hash = 0;
+    for (int base = (blockIdx.x * kOccNetWarps + warp) * 32; base < n; base += gridDim.x * kOccNetWarps * 32) {
+        const int r = base + lane;
+        int cell = -1;
+        __half2* arow = reinterpret_cast<__half2*>(&At[warp][lane][0]);
+        if (r < n) {
+            const float4 v = reinterpret_cast<const float4*>(a.roots)[r];
+            cell = __float_as_int(v.w);
+            // ngp.py:75,77: x = (x - center) / scale + 0.5 ; clamp [0,1]
+            const float n0 = fminf(fmaxf((v.x - cs[0]) / cs[3] + 0.5f, 0.f), 1.f);
+            const float n1 = fminf(fmaxf((v.y - cs[1]) / cs[4] + 0.5f, 0.f), 1.f);
+            const float n2 = fminf(fmaxf((v.z - cs[2]) / cs[5] + 0.5f, 0.f), 1.f);
+#pragma unroll 4
+            for (int l = 0; l < kLevels; l++) arow[l] = hash_encode_level(table, a.sd.hl, l, n0, n1, n2, &st_hash);
+        } else {
+#pragma unroll
+            for (int l = 0; l < kLevels; l++) arow[l] = __floats2half2_rn(0.f, 0.f);
+        }
+        __syncwarp();
+#pragma unroll
+        for (int mt = 0; mt < 2; mt++) {
+            float o[2][4];
+            mlp_density_tile16(&At[warp][16 * mt][0], W, lane, o);
+            const int cA = __shfl_sync(kFull, cell, 16 * mt + g), cB = __shfl_sync(kFull, cell, 16 * mt + g + 8);
+            if (t == 0) {
+                // sigma = column 0 rounded to fp16 (tcnn's fp16 output), as mlp_tile16 takes it
+                float s[2] = {__low2float(__floats2half2_rn(o[0][0], o[0][1])), __low2float(__floats2half2_rn(o[0][2], o[0][3]))};
+                const int c[2] = {cA, cB};
+#pragma unroll
+                for (int h = 0; h < 2; h++) {
+                    if (kNanToNum && !isfinite(s[h])) s[h] = 0.f;  // snarf_deformer.py:137-138 nan_to_num(x, 0, 0, 0)
+                    // positive densities are ~2 % of the cells: with peer pointers the cross-GPU max-reduction is these
+                    // few atomics over NVLink instead of a 1 MB all-reduce after the kernel
+                    if (c[h] >= 0 && s[h] > 0.f) {
+                        if (a.peer_density) {
+                            for (int pr = 0; pr < a.n_peers; pr++) atomicMax(reinterpret_cast<int*>(a.peer_density[pr]) + c[h], __float_as_int(s[h]));
+                        } else {
+                            atomicMax(reinterpret_cast<int*>(a.density_max) + c[h], __float_as_int(s[h]));
+                        }
+                    }
+                }
+            }
+        }
+        __syncwarp();
+    }
+    if (a.stats) {
+#pragma unroll
+        for (int o = 16; o; o >>= 1) st_hash += __shfl_xor_sync(kFull, st_hash, o);
+        if (lane == 0) atomicAdd(&a.stats->hash_loads, (unsigned long long)st_hash);
     }
 }
 
@@ -977,7 +1124,7 @@ static int launch_query_t(QueryArgs& a, cudaStream_t stream) {
         IA_CHECK_CUDA(cudaFuncSetAttribute(deform_query_kernel<kWarps, kKeepXc, kNV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
         attr_set.set();
     }
-    const int n_batches = a.grid_aabb ? (a.G * a.G * a.G + (32 / a.passes) - 1) / (32 / a.passes) : (a.n + 31) / 32;
+    const int n_batches = (a.n + 31) / 32;
     int grid = sm_count();
     if (grid <= 0) return set_err(IA_ECUDA, "no CUDA device%s");
     grid = min(grid, (n_batches + kWarps - 1) / kWarps);
@@ -993,7 +1140,6 @@ static int launch_query(QueryArgs& a, cudaStream_t stream) {
         return launch_query_t<12, false, true>(a, stream);
     }
     if (a.xc_best) return launch_query_t<12, true>(a, stream);
-    // 16 warps measured ~1 % faster than 12 for the occupancy passes on an H100 (DESIGN §5.2); the default is still 12
     if (g_query_warps == 16) return launch_query_t<16, false>(a, stream);
     return launch_query_t<12, false>(a, stream);
 }
@@ -1067,9 +1213,7 @@ int ia_deform_query(const IaScene* scene, const float* pts, int n, int eval_mode
     if (rc) return rc;
     a.pts = pts; a.n = n; a.eval_mode = eval_mode; a.rgb = rgb; a.sigma = sigma; a.xc_best = xc_best;
     a.best_init = best_init; a.stats = stats;
-    a.grid_jitter = nullptr; a.grid_aabb = nullptr; a.G = 0; a.density_max = nullptr; a.passes = 1;
-    a.batch_counter = nullptr; a.batch_first = 0; a.batch_stride = 1;
-    a.peer_density = nullptr; a.n_peers = 0;
+    a.batch_counter = nullptr;
     a.n_dev = nullptr; a.index = nullptr; a.lanes_per_sample = 1;
     return launch_query(a, (cudaStream_t)stream);
 }
@@ -1087,9 +1231,7 @@ __attribute__((visibility("hidden"))) int ia_internal_query_list(const IaScene* 
     if (rc) return rc;
     a.pts = pts; a.n = capacity; a.eval_mode = eval_mode; a.rgb = rgb; a.sigma = sigma; a.xc_best = xc_best;
     a.best_init = best_init; a.stats = stats;
-    a.grid_jitter = nullptr; a.grid_aabb = nullptr; a.G = 0; a.density_max = nullptr; a.passes = 1;
-    a.batch_counter = batch_counter; a.batch_first = 0; a.batch_stride = 1;
-    a.peer_density = nullptr; a.n_peers = 0;
+    a.batch_counter = batch_counter;
     a.n_dev = n_dev; a.index = index; a.lanes_per_sample = g_query_lanes;
     return launch_query(a, (cudaStream_t)stream);
 }
@@ -1097,26 +1239,46 @@ __attribute__((visibility("hidden"))) int ia_internal_query_list(const IaScene* 
 static int occupancy_query_impl(const IaScene* scene, const float* jitter, const float* aabb, int G, int passes,
                                 float* density_max, float* const* peer_density, int n_peers, void* workspace, int shard,
                                 int n_shards, IaStats* stats, ia_stream_t stream) {
-    IA_REQUIRE(jitter && aabb && (density_max || peer_density) && G > 0 && passes > 0 && passes <= 32);
+    IA_REQUIRE(jitter && aabb && (density_max || peer_density) && workspace && G > 0 && G <= 1024 && passes > 0 && passes <= 32);
     IA_REQUIRE(n_shards >= 1 && shard >= 0 && shard < n_shards);
-    QueryArgs a;
+    OccArgs a;
     int rc = make_scene_dev(scene, a.sd, false);
     if (rc) return rc;
-    a.pts = nullptr; a.n = passes * G * G * G; a.eval_mode = 1; a.rgb = nullptr; a.sigma = nullptr; a.xc_best = nullptr;
-    a.best_init = nullptr; a.stats = stats;
-    a.grid_jitter = jitter; a.grid_aabb = aabb; a.G = G; a.density_max = density_max; a.passes = passes;
-    a.batch_counter = reinterpret_cast<int*>(workspace);
+    a.grid_jitter = jitter; a.grid_aabb = aabb; a.G = G; a.passes = passes;
+    a.counters = reinterpret_cast<int*>(workspace);
+    a.cand = reinterpret_cast<float*>(reinterpret_cast<char*>(workspace) + 256);
+    a.roots = reinterpret_cast<OccRoot*>(reinterpret_cast<char*>(workspace) + kOccCandBytes);
     a.batch_first = shard; a.batch_stride = n_shards;
-    a.peer_density = peer_density; a.n_peers = n_peers;
-    a.n_dev = nullptr; a.index = nullptr;
+    a.density_max = density_max; a.peer_density = peer_density; a.n_peers = n_peers;
+    a.stats = stats;
+    cudaStream_t st = (cudaStream_t)stream;
+    const int sms = sm_count();
+    if (sms <= 0) return set_err(IA_ECUDA, "no CUDA device%s");
+    IA_CHECK_CUDA(cudaMemsetAsync(workspace, 0, 256, st));
+    // peer mode: every rank's buffer is written by all ranks -- the CALLER zeroes it (before the barrier that precedes this launch)
+    if (!peer_density) IA_CHECK_CUDA(cudaMemsetAsync(density_max, 0, sizeof(float) * G * G * G, st));
     // one lane per point: unlike in the training list query, several lanes per point do not pay here -- 98 % of the grid
     // points are empty space whose solves end after one or two gathers, so splitting a point's 13 solves over lanes
-    // shortens nothing and idles the helper lanes in every later stage
-    a.lanes_per_sample = 1;
-    if (workspace) IA_CHECK_CUDA(cudaMemsetAsync(workspace, 0, 256, (cudaStream_t)stream));
-    // peer mode: every rank's buffer is written by all ranks -- the CALLER zeroes it (before the barrier that precedes this launch)
-    if (!peer_density) IA_CHECK_CUDA(cudaMemsetAsync(density_max, 0, sizeof(float) * G * G * G, (cudaStream_t)stream));
-    return launch_query(a, (cudaStream_t)stream);
+    // shortens nothing
+    const int n_batches = (occ_batches(G, passes) - shard + n_shards - 1) / n_shards;
+    const int roots_grid = min(min(sms * kOccRootCtas, kOccRootMaxCtas), (n_batches + kOccRootWarps - 1) / kOccRootWarps);
+    if (roots_grid > 0) {
+        if (scene->nv) occupancy_roots_kernel<true><<<roots_grid, kOccRootWarps * 32, 0, st>>>(a);
+        else occupancy_roots_kernel<false><<<roots_grid, kOccRootWarps * 32, 0, st>>>(a);
+        IA_CHECK_CUDA(cudaPeekAtLastError());
+    }
+    // the root count stays on the device (the frame is one CUDA graph): a persistent grid strides over the list
+    if (scene->nv) occupancy_net_kernel<false><<<sms * kOccNetCtas, kOccNetWarps * 32, 0, st>>>(a);
+    else occupancy_net_kernel<true><<<sms * kOccNetCtas, kOccNetWarps * 32, 0, st>>>(a);
+    IA_CHECK_CUDA(cudaPeekAtLastError());
+    return IA_OK;
+}
+
+extern "C" size_t ia_occupancy_query_workspace_bytes(int G, int passes, int n_shards) {
+    if (G <= 0 || G > 1024 || passes <= 0 || passes > 32 || n_shards < 1) return 0;
+    // worst case: every kept candidate of every grid point of the shard's batches survives the filter
+    const long batches = (occ_batches(G, passes) + n_shards - 1) / n_shards;
+    return kOccCandBytes + sizeof(OccRoot) * (size_t)batches * (size_t)(occ_cells_per_batch(passes) * passes) * kNumInit;
 }
 
 extern "C" int ia_occupancy_query(const IaScene* scene, const float* jitter, const float* aabb, int G, int passes,

@@ -62,12 +62,13 @@ __device__ __forceinline__ int warp_excl_scan(int v, int lane, int& total) {
     return x - v;
 }
 
-template <bool kKeepXc>
-__device__ __forceinline__ void warp_eval_samples(const EvalCtx& ctx, WarpScratch<kKeepXc>& ws, bool active, float xd0,
-                                                  float xd1, float xd2, bool eval_mode, int lane, SampleOut& out,
-                                                  unsigned& ngather, unsigned& nroots, unsigned& nload, unsigned& nhash,
-                                                  const int lanes_per_sample = 1) {
-    const FrameConst& fc = *ctx.fc;
+// Steps 1-2 of warp_eval_samples, shared with the occupancy pass's root-finding kernel: the 13 Broyden solves of the
+// lane's sample into cand[3][kNumInit][lane] and the duplicate filter; returns the mask of the kept roots.
+// kStoreAll = false stores converged candidates only: the filter and the kept roots read no others.
+template <bool kStoreAll = true>
+__device__ __forceinline__ unsigned warp_find_roots(const FieldDesc& field, const FrameConst& fc, float (*cand)[kNumInit][32],
+                                                    bool active, float xd0, float xd1, float xd2, int lane, unsigned& ngather,
+                                                    unsigned& nload, const int lanes_per_sample = 1) {
     // ---- 1. Broyden from the 13 bone initialisations ------------------------------------------------
     // lanes_per_sample k in {1, 2, 4}: the warp holds 32/k samples (lanes 0 .. 32/k-1 own them, lane l + j*32/k helps
     // sample l and must be given the same point and `active`); the 13 solves of a sample are dealt round-robin to its k
@@ -81,12 +82,14 @@ __device__ __forceinline__ void warp_eval_samples(const EvalCtx& ctx, WarpScratc
         if (active) {
             float x[3];
             int ng = 0;
-            const bool ok = broyden_solve(ctx.field, fc.bp, fc.Tb[b], xd0, xd1, xd2, x, nullptr, ng);
+            const bool ok = broyden_solve(field, fc.bp, fc.Tb[b], xd0, xd1, xd2, x, nullptr, ng);
             ngather += ng & 0xffff;
             nload += (unsigned)ng >> 16;
-            ws.cand[0][b][sl0] = x[0];
-            ws.cand[1][b][sl0] = x[1];
-            ws.cand[2][b][sl0] = x[2];
+            if (kStoreAll || ok) {
+                cand[0][b][sl0] = x[0];
+                cand[1][b][sl0] = x[1];
+                cand[2][b][sl0] = x[2];
+            }
             if (ok) vmask |= 1u << b;
         }
     }
@@ -101,15 +104,25 @@ __device__ __forceinline__ void warp_eval_samples(const EvalCtx& ctx, WarpScratc
 #pragma unroll 1
         for (int i = 0; i < kNumInit - 1; i++) {
             if (!((vmask >> i) & 1)) continue;
-            const float xi0 = ws.cand[0][i][lane], xi1 = ws.cand[1][i][lane], xi2 = ws.cand[2][i][lane];
+            const float xi0 = cand[0][i][lane], xi1 = cand[1][i][lane], xi2 = cand[2][i][lane];
 #pragma unroll 1
             for (int j = i + 1; j < kNumInit; j++) {
                 if (!((vmask >> j) & 1)) continue;
-                const float d0 = xi0 - ws.cand[0][j][lane], d1 = xi1 - ws.cand[1][j][lane], d2 = xi2 - ws.cand[2][j][lane];
+                const float d0 = xi0 - cand[0][j][lane], d1 = xi1 - cand[1][j][lane], d2 = xi2 - cand[2][j][lane];
                 if (dot3f(d0, d0, d1, d1, d2, d2) < fc.filter_thr) { kept &= ~(1u << i); break; }
             }
         }
     }
+    return kept;
+}
+
+template <bool kKeepXc>
+__device__ __forceinline__ void warp_eval_samples(const EvalCtx& ctx, WarpScratch<kKeepXc>& ws, bool active, float xd0,
+                                                  float xd1, float xd2, bool eval_mode, int lane, SampleOut& out,
+                                                  unsigned& ngather, unsigned& nroots, unsigned& nload, unsigned& nhash,
+                                                  const int lanes_per_sample = 1) {
+    const FrameConst& fc = *ctx.fc;
+    const unsigned kept = warp_find_roots(ctx.field, fc, ws.cand, active, xd0, xd1, xd2, lane, ngather, nload, lanes_per_sample);
     // ---- 3. compact surviving roots into the warp's root list --------------------------------------
     int total;
     int pos = warp_excl_scan(__popc(kept), lane, total);

@@ -1,6 +1,7 @@
 """Host-side mirror of instant_avatar/models/structures/density_grid.py::DensityGrid (64^3 occupancy grid).
 
-The per-cell density queries run through the fused point-query kernel (`deformer(coords, net, eval_mode)`); the grid
+The per-cell density queries run through the fused point-query kernel (`deformer(coords, net, eval_mode)`, train-time
+refresh) and the occupancy-pass kernels (`ops.occupancy_query`, per-frame initialisation); the grid
 post-processing (EMA, 1-exp, 3x3x3 dilation, threshold, largest 26-connected component) runs in the
 `ia_occupancy_*` kernels when available and otherwise in the PyTorch ops the reference uses.
 """
@@ -112,18 +113,23 @@ class DensityGrid(torch.nn.Module):
         self.aabb = deformer.get_bbox_deformed()
         from ..networks.ngp import NeRFNGPNet
         if isinstance(net, NeRFNGPNet) and hasattr(deformer, "scene") and getattr(deformer, "fusable", True):
-            # all passes in one launch of the fused point-query kernel (points generated from the cell index)
+            # all passes in one occupancy pass (points generated from the cell index): root finding, then the network
             if jitters is None:
                 jitters = torch.rand((iters, *self.coords.shape), device=self.coords.device)
             net.initialize(deformer.bbox)
+            # the root list of the pass, allocated once (CUDA-graph replays keep its address)
+            nbytes = ops.occupancy_query_workspace_bytes(self.grid_size, iters, shard[1])
+            if getattr(self, "_qws", None) is None or self._qws.numel() < nbytes:
+                self._qws = torch.empty(nbytes, device=self.coords.device, dtype=torch.uint8)
             if peer is not None:
-                ops.occupancy_query(deformer.scene(net), jitters[:iters], self.aabb6(), shard=shard, peer=peer.density_ptrs)
+                ops.occupancy_query(deformer.scene(net), jitters[:iters], self.aabb6(), workspace=self._qws, shard=shard,
+                                    peer=peer.density_ptrs)
                 peer.barrier_density()
                 self.build_from_density(peer.density)
                 peer.density.zero_()   # own buffer, for the next frame: nobody writes into it before the frame-end barrier
                 return
             self._density = ops.occupancy_query(deformer.scene(net), jitters[:iters], self.aabb6(), getattr(self, "_density", None),
-                                                shard=shard)
+                                                workspace=self._qws, shard=shard)
             if shard[1] > 1:
                 import torch.distributed as dist
                 dist.all_reduce(self._density, op=dist.ReduceOp.MAX)

@@ -113,13 +113,24 @@ def mc_largest_component(verts: torch.Tensor, faces: torch.Tensor):
     return verts_out[:kv], faces_out[:kf]
 
 
+def occupancy_query_workspace_bytes(G: int, passes: int, n_shards: int = 1) -> int:
+    """bytes of the occupancy pass's workspace: counters and the root list, which holds the worst case of the shard
+    (every one of a grid point's 13 root finds kept)"""
+    return int(lib().ia_occupancy_query_workspace_bytes(C.c_int(G), C.c_int(passes), C.c_int(n_shards)))
+
+
 def occupancy_query(scene, jitters: torch.Tensor, aabb6: torch.Tensor, density=None, stats=None, workspace=None, shard=(0, 1), peer=None):
-    """5-pass density query of DensityGrid.initialize in one launch -> density [G,G,G] (max over passes, >= 0).
+    """5-pass density query of DensityGrid.initialize -> density [G,G,G] (max over passes, >= 0): root finding, then the
+    network on the list of kept roots.  workspace: uint8 device buffer of occupancy_query_workspace_bytes(G, passes,
+    n_shards) bytes or more (allocated per call when None).
     peer = (device address of the array of every rank's density pointer, n_ranks): this rank's shard is max-reduced into
     all ranks' (pre-zeroed) buffers with NVLink atomics; returns None (the caller owns the symmetric buffer)."""
     P, G = jitters.shape[0], jitters.shape[1]
+    nbytes = occupancy_query_workspace_bytes(G, P, shard[1])
     if workspace is None:
-        workspace = torch.empty(64, device=jitters.device, dtype=torch.int32)
+        workspace = torch.empty(nbytes, device=jitters.device, dtype=torch.uint8)
+    if workspace.numel() * workspace.element_size() < nbytes:
+        raise ValueError(f"occupancy_query: workspace of {workspace.numel() * workspace.element_size()} bytes, needs {nbytes}")
     s = scene.c_struct()
     if peer is not None:
         _lib.count(1); check(lib().ia_occupancy_query_peer(C.byref(s), ptr(jitters.contiguous(), f32), ptr(aabb6, f32), C.c_int(G), C.c_int(P),
