@@ -583,6 +583,35 @@ int ia_smpl_fit_forward(const IaSmplModel* model /*[host]*/, const float* params
 int ia_smpl_fit_objective(const IaSmplModel* model /*[host]*/, const IaKeypointFit* fit /*[host]*/, const float* params, int F,
                           void* workspace, size_t workspace_bytes, float* loss, float* grad, ia_stream_t stream);
 
+/* Hard rasterisation and headlight shading of F posed meshes that share one face list, composited over the frames:
+ * visualize-SMPL.py's overlay video (DESIGN.md §3.4, §5.11).  fp32 throughout.
+ *
+ * verts [F][V][3] (device, world space), faces [NF][3] int32 (device; a face with an index outside [0, V) is not drawn),
+ * K [3][3] and E [4][4] (HOST, row-major; the cameras.npz intrinsic / extrinsic, only E's first three rows are read).
+ * workspace: device, 16-byte aligned, ia_raster_workspace_bytes(F, V, NF) bytes (0 for invalid sizes), shared by both
+ * calls.  No host synchronisation; two calls on the same input give bit-identical results.
+ *
+ * ia_raster: per frame f and pixel (row r, column j), sampled at the image point (u, v) = (j, r) with
+ *   [u v 1]^T ~ K (R x + t): face_id [F][H][W] int32 (-1: none), depth [F][H][W] (camera-space z = 1 / sum_i b_i / z_i of
+ *   the screen-space barycentrics b_i; 0 where face_id = -1) and bary [F][H][W][2] (the perspective-correct barycentrics of
+ *   faces[id][1] and faces[id][2]; 8-byte aligned).  Coverage: all three edge functions >= 0 at the sample point after
+ *   orienting the face (both windings drawn).  Visibility: the smallest depth, ties to the lowest face index.  Not drawn: a
+ *   face with a vertex at camera z <= 0.01, a face of zero screen area, a fragment with z > 8.
+ * ia_shade_composite: frames [F][H][W][3] uint8 (device, BGR, in place): each pixel with a face becomes
+ *   uint8(min(255, floor(255 c + 0.5))), c = albedo (ka + kd |n . l|), with n the perspective-correct interpolation of the
+ *   normalised vertex normals (area-weighted face normals summed in the order of the vertex -> face CSR csr_offsets [V+1],
+ *   csr_faces [csr_offsets[V]], device int32) and l the unit view ray of the pixel; face_id and bary as ia_raster wrote them.
+ * IA_EINVAL: F outside [0, 65535], a negative V or NF, H or W outside [1, 16384], a singular K, a short workspace, a NULL
+ * pointer. */
+size_t ia_raster_workspace_bytes(int F, int n_verts, int n_faces);
+int ia_raster(const float* verts, int F, int n_verts, const int* faces, int n_faces, const float* K /*[host]*/,
+              const float* E /*[host]*/, int H, int W, void* workspace, size_t workspace_bytes, int* face_id, float* depth,
+              float* bary, ia_stream_t stream);
+int ia_shade_composite(const float* verts, int F, int n_verts, const int* faces, int n_faces, const int* csr_offsets,
+                       const int* csr_faces, const float* K /*[host]*/, const float* E /*[host]*/, int H, int W,
+                       const int* face_id, const float* bary, void* workspace, size_t workspace_bytes, uint8_t* frames,
+                       ia_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -5,6 +5,7 @@ from __future__ import annotations
 import ctypes as C
 from dataclasses import dataclass, field as dc_field
 
+import numpy as np
 import torch
 
 from . import _lib
@@ -893,6 +894,70 @@ def smpl_fit_objective(model: SmplFitModel, params, F: int, keypoints, proj, joi
     fit.threshold = float(threshold)
     _lib.count(13); check(lib().ia_smpl_fit_objective(C.byref(s), C.byref(fit), ptr(params, f32), C.c_int(F), ptr(workspace),
                                                       C.c_size_t(workspace.numel()), ptr(loss, f32), ptr(grad, f32), stream()))
+
+
+def face_csr(faces, n_verts: int, device):
+    """Vertex -> face CSR of a face list [NF,3] for shade_composite: (offsets [V+1], face ids [3NF]) int32 on `device`,
+    each vertex's faces in ascending index.  Built on the host once per face list."""
+    f = np.asarray(faces.cpu() if torch.is_tensor(faces) else faces).reshape(-1, 3).astype(np.int64)
+    if f.size and (f.min() < 0 or f.max() >= n_verts):
+        raise ValueError(f"faces: indices must lie in [0, {n_verts})")
+    order = np.argsort(f.ravel(), kind="stable")
+    offsets = np.zeros(n_verts + 1, np.int64)
+    np.cumsum(np.bincount(f.ravel(), minlength=n_verts), out=offsets[1:])
+    t = lambda a: torch.from_numpy(a.astype(np.int32)).to(device)
+    return t(offsets), t(order // 3)
+
+
+def raster_workspace(F: int, n_verts: int, n_faces: int, device) -> torch.Tensor:
+    nbytes = int(lib().ia_raster_workspace_bytes(C.c_int(F), C.c_int(n_verts), C.c_int(n_faces)))
+    if nbytes == 0 and F > 0:
+        raise ValueError(f"raster: invalid sizes F={F} V={n_verts} NF={n_faces}")
+    return torch.empty(max(nbytes, 16), device=device, dtype=torch.uint8)
+
+
+def _camera(K, E):
+    K = np.asarray(K, np.float64)
+    E = np.asarray(E, np.float64)
+    if K.shape != (3, 3) or E.shape not in ((4, 4), (3, 4)):
+        raise ValueError(f"raster: K must be [3,3] and E [4,4], got {K.shape} and {E.shape}")
+    return (C.c_float * 9)(*K.ravel().tolist()), (C.c_float * 12)(*E[:3].ravel().tolist())
+
+
+def rasterize(verts, faces, K, E, H: int, W: int, workspace=None):
+    """Hard rasterisation of F posed meshes sharing one face list (include/ia_b200.h, ia_raster; DESIGN.md §3.4):
+    verts [F,V,3] fp32, faces [NF,3] int32 (device), K [3,3] / E [4,4] (host) -> dict of face_id [F,H,W] int32 (-1: none),
+    depth [F,H,W] and bary [F,H,W,2] (perspective-correct barycentrics of faces[:,1] and faces[:,2]).  Two launches, no
+    host synchronisation."""
+    F, V = verts.shape[0], verts.shape[1]
+    NF = faces.shape[0]
+    dev = verts.device
+    workspace = raster_workspace(F, V, NF, dev) if workspace is None else workspace
+    out = {"face_id": torch.empty((F, H, W), device=dev, dtype=torch.int32),
+           "depth": torch.empty((F, H, W), device=dev, dtype=f32),
+           "bary": torch.empty((F, H, W, 2), device=dev, dtype=f32)}
+    Kc, Ec = _camera(K, E)
+    _lib.count(2); check(lib().ia_raster(ptr(verts, f32), C.c_int(F), C.c_int(V), ptr(faces, torch.int32), C.c_int(NF), Kc, Ec,
+                                         C.c_int(H), C.c_int(W), ptr(workspace), C.c_size_t(workspace.numel()),
+                                         ptr(out["face_id"]), ptr(out["depth"]), ptr(out["bary"]), stream()))
+    return out
+
+
+def shade_composite(frames, verts, faces, csr, raster: dict, K, E, workspace=None):
+    """Headlight shading of rasterize's output over frames [F,H,W,3] uint8 (device, BGR), in place (ia_shade_composite;
+    DESIGN.md §3.4): pixels with a face get the mesh's colour, the rest keep the frame.  csr: face_csr(faces).  Two
+    launches, no host synchronisation.  -> frames"""
+    F, H, W = raster["face_id"].shape
+    if frames.dtype != torch.uint8 or tuple(frames.shape) != (F, H, W, 3):
+        raise ValueError(f"shade_composite: frames must be uint8 {(F, H, W, 3)}, got {frames.dtype} {tuple(frames.shape)}")
+    V, NF = verts.shape[1], faces.shape[0]
+    workspace = raster_workspace(F, V, NF, verts.device) if workspace is None else workspace
+    Kc, Ec = _camera(K, E)
+    _lib.count(2); check(lib().ia_shade_composite(ptr(verts, f32), C.c_int(F), C.c_int(V), ptr(faces, torch.int32), C.c_int(NF),
+                                                  ptr(csr[0], torch.int32), ptr(csr[1], torch.int32), Kc, Ec, C.c_int(H),
+                                                  C.c_int(W), ptr(raster["face_id"], torch.int32), ptr(raster["bary"], f32),
+                                                  ptr(workspace), C.c_size_t(workspace.numel()), ptr(frames), stream()))
+    return frames
 
 
 # ------------------------------------------------------------------------------------------------------------------
