@@ -134,3 +134,74 @@ def test_keypoint_shape_mismatch_is_refused(golden, tmp_path, shape):
     write_folder(str(tmp_path), golden, kp=np.zeros(shape, np.float32))
     with pytest.raises(ValueError, match="keypoints.npy"):
         refine_smpl.refine_sequence(str(tmp_path), smpl_data=synthetic.smpl_dict_cached(0))
+
+
+@pytest.mark.parametrize("F", [2, 3, 31, 33, 65])
+def test_sequence_plants_its_edges(F):
+    """refine_smpl_ref.sequence: on the first and last frames of the 32-frame tiles (the middle frames when F <= 32),
+    confidences of exactly float32(0.2) are masked by the objective and their nextafter neighbours are not, the
+    rotation vectors have the stated magnitudes, the repeated frames give a regulariser residual of exactly 0, and the
+    masked frame has no keypoint left"""
+    start, kp, proj = refine_smpl_ref.sequence(F, seed=F)
+    tables = refine_smpl.load_tables()
+    edges = refine_smpl_ref.edge_frames(F)
+    if F > refine_smpl_ref.FT:
+        assert edges == sorted({f for t in range(0, F, 32) for f in (t, min(t + 31, F - 1))})
+    assert all(v.dtype == np.float32 for v in start.values()) and kp.dtype == np.float32 and kp.shape == (F, 25, 3)
+    for f in edges:
+        for j, mag in refine_smpl_ref.ROT_EDGES:
+            assert abs(np.linalg.norm(start["body_pose"][f, 3 * (j - 1):3 * j].astype(np.float64)) - mag) <= 1e-6 * mag
+    assert (start["global_orient"][edges[-1]] == 0).all()
+
+    model = refine_smpl_ref.smpl64(synthetic.smpl_dict_cached(0))
+    t = {k: torch.tensor(v, dtype=torch.float64).reshape((1, 10) if k == "betas" else v.shape) for k, v in start.items()}
+    kp_term = lambda k: refine_smpl_ref.objective(model, t, k, proj, tables, 0.2)[1].item()
+    a = refine_smpl_ref.repeated_pair(F)
+    verts = refine_smpl_ref.objective(model, t, kp, proj, tables, 0.2)[4]
+    assert (verts[a + 1] - verts[a] == 0).all()
+    assert F == 2 or (verts[a + 1] != verts[a - 1 if a > 0 else a + 2]).any()  # only that pair
+    mf = refine_smpl_ref.masked_frame(F)
+    assert (mf is None) == (F == 2)
+    if mf is not None:
+        assert 0 < mf < F - 1 and (kp[mf, :, 2] == 0).all()
+    zero = kp.copy()
+    n_at = n_above = 0
+    for i, f in enumerate(edges):
+        at, above = refine_smpl_ref.threshold_joints(i)
+        if f == mf:
+            continue
+        assert (kp[f, at, 2] == np.float32(0.2)).all() and (kp[f, above, 2] == np.nextafter(np.float32(0.2), np.float32(1))).all()
+        zero[f, at, 2] = 0.0
+        n_at += len(at)
+        n_above += sum(1 for j in above if j in tables["select_joints"])
+    assert n_at > 0 and n_above > 0
+    base = kp_term(kp)
+    assert kp_term(zero) == base  # the exact threshold is masked
+    for i, f in enumerate(edges):  # each kept neighbour counts
+        if f != mf:
+            for j in refine_smpl_ref.threshold_joints(i)[1]:
+                if j in tables["select_joints"]:
+                    k = kp.copy(); k[f, j, 2] = 0.0
+                    assert kp_term(k) < base, (f, j)
+
+
+def test_per_frame_betas_contributions_sum_to_the_betas_gradient():
+    start, kp, proj = refine_smpl_ref.sequence(40, seed=1)
+    model = refine_smpl_ref.smpl64(synthetic.smpl_dict_cached(0))
+    tables = refine_smpl.load_tables()
+    loss, g = refine_smpl_ref.g64(model, start, kp, proj, tables)
+    loss_c, c = refine_smpl_ref.c64(model, start, kp, proj, tables)
+    assert c["betas"].shape == (40, 10) and loss_c == loss
+    assert np.abs(c["betas"].sum(0) - g["betas"]).max() <= 1e-12 * np.abs(g["betas"]).max()
+    for k in ("global_orient", "body_pose", "transl"):
+        assert np.abs(c[k].reshape(g[k].shape) - g[k]).max() <= 1e-12 * np.abs(g[k]).max(), k
+
+
+def test_300_frame_float64_objective_is_finite():
+    """the long sequence, with its repeated frames (a zero regulariser residual), gives a finite loss and gradient"""
+    start, kp, proj = refine_smpl_ref.sequence(300, seed=300)
+    loss, g = refine_smpl_ref.g64(refine_smpl_ref.smpl64(synthetic.smpl_dict_cached(0)), start, kp, proj,
+                                  refine_smpl.load_tables())
+    assert np.isfinite(loss) and loss > 0
+    for k, v in g.items():
+        assert np.isfinite(v).all(), k
