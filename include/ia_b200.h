@@ -46,7 +46,8 @@ typedef struct IaNearestVertex {
 
 /* Per-frame read-only state of the fused kernels. */
 typedef struct IaScene {
-    const float* field;      /* [D][H][W][24] fp32: blended 3x4 LBS transform of voxel x followed by that of voxel x+1 (zeros at x = W-1); 96-B records written by ia_precompute */
+    const float* field;      /* [D][H][W+1][12] fp32 written by ia_precompute: the blended 3x4 LBS transform (row-major) of each voxel
+                              * once, rows padded with one zero voxel; the 24 floats from voxel x on are voxel x, then voxel x+1 */
     int32_t D, H, W;
     const float* offset_k;   /* [3] ForwardDeformer.offset_kernel (deformer_torch.py:154) */
     const float* scale_k;    /* [3] ForwardDeformer.scale_kernel  (deformer_torch.py:155-158) */
@@ -71,7 +72,7 @@ typedef struct IaStats {
     unsigned long long gathers;   /* trilinear field samples taken by Broyden (M*13*kbar) */
     unsigned long long net_evals; /* hash-grid + MLP evaluations (P) */
     unsigned long long rays_hit;  /* rays with at least one occupied sample */
-    unsigned long long field_loads; /* of `gathers`, those that issued loads (12 sectors of 32 B each): footprints outside the
+    unsigned long long field_loads; /* of `gathers`, those that issued loads (4 x-pairs of 96 B each, counted as 12 sectors of 32 B): footprints outside the
                                      * skinning volume and early-out solves are exact zeros computed without memory traffic */
     unsigned long long hash_loads; /* hash-table loads issued per lane (one 32-byte sector each): 16 levels x 8 corners = 128 per
                                     * network evaluation */
@@ -94,7 +95,8 @@ int ia_hashgrid_layout(uint32_t res[IA_NUM_LEVELS], float scale[IA_NUM_LEVELS], 
 
 /* Replaces precompute_cuda.precompute (deformers/fast_snarf/cuda/precompute/precompute.cpp:7-13,
  * precompute.cu:24-103).  voxel_w [24][D][H][W] skinning weights, tfs [24][4][4].
- * field_out [D][H][W][24] (x-pair records: row-major 3x4 of voxel x, then of voxel x+1; 32-byte aligned); voxel_d_out [3][D][H][W] (nullable; reference layout, deformer.voxel_d);
+ * field_out [D][H][W+1][12]: D*H*(W+1)*12 floats, 16-byte aligned (a larger buffer works too), the row-major 3x4 of every voxel
+ * and a zero voxel at the end of each row (IaScene.field); voxel_d_out [3][D][H][W] (nullable; reference layout, deformer.voxel_d);
  * aabb_out [6] = min/max of voxel_d (nullable; SNARFDeformer.get_bbox_deformed, snarf_deformer.py:105-107). */
 int ia_precompute(const float* voxel_w, const float* tfs, const float* offset_k, const float* scale_k, int D, int H,
                   int W, float* field_out, float* voxel_d_out, float* aabb_out, ia_stream_t stream);
@@ -252,10 +254,10 @@ int ia_occupancy_query_peer(const IaScene* scene /*[host]*/, const float* jitter
                             IaStats* stats, ia_stream_t stream);
 
 /* Measurement aid (bench.py `roofline.peak`): the fused kernels' memory access shape in isolation -- every lane gathers
- * trilinear footprints (4 x-pair records = 12 x 32-byte sectors, 12 LDG.E.256) from the L2-resident field `field`
- * [D][H][W][24], the next footprint depending on the loaded data -- at one persistent CTA of `warps` (12 / 16 / 24 / 32)
+ * trilinear footprints (4 x-pairs of 96 B = 24 LDG.128, 3-4 32-byte sectors per pair) from the L2-resident field `field`
+ * (IaScene.field layout), the next footprint depending on the loaded data -- at one persistent CTA of `warps` (12 / 16 / 24 / 32)
  * warps per SM.  coherent != 0: the lanes of a warp stay within a 10 x 3 x 3 voxel neighbourhood (a batch of the
- * occupancy query).  *sectors_out (device) += sectors requested; the caller times the launch with CUDA events. */
+ * occupancy query).  *sectors_out (device) += 12 sectors per footprint (nominal, 3 per pair); the caller times the launch with CUDA events. */
 int ia_gather_ceiling(const float* field, int D, int H, int W, int iters, int warps, int coherent,
                       unsigned long long* sectors_out, float* sink /*nullable*/, ia_stream_t stream);
 

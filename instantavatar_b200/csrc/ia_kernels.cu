@@ -870,7 +870,7 @@ __device__ __forceinline__ void atomic_max_f(float* addr, float v) {
 __global__ void __launch_bounds__(256) precompute_kernel(const float* __restrict__ voxel_w, const float* __restrict__ tfs,
                                                          const float* __restrict__ offset_k,
                                                          const float* __restrict__ scale_k, int D, int H, int W,
-                                                         float4* __restrict__ field, float* __restrict__ voxel_d,
+                                                         float* __restrict__ field, float* __restrict__ voxel_d,
                                                          float* __restrict__ aabb) {
     __shared__ float T[24][12];
     __shared__ float red[6];
@@ -897,20 +897,15 @@ __global__ void __launch_bounds__(256) precompute_kernel(const float* __restrict
 #pragma unroll
             for (int c = 0; c < 12; c++) J[c] = __fmaf_rn(w, T[j][c], J[c]);
         }
-        // x-pair records (ia_device.cuh): slot A of this voxel's record, slot B of its -x neighbour's record; the last
-        // voxel of a row has a zero-filled slot B (the padding neighbour, weight 0 in the sampler)
-        field[index * 6 + 0] = make_float4(J[0], J[1], J[2], J[3]);
-        field[index * 6 + 1] = make_float4(J[4], J[5], J[6], J[7]);
-        field[index * 6 + 2] = make_float4(J[8], J[9], J[10], J[11]);
-        if (idx_w > 0) {
-            field[(index - 1) * 6 + 3] = make_float4(J[0], J[1], J[2], J[3]);
-            field[(index - 1) * 6 + 4] = make_float4(J[4], J[5], J[6], J[7]);
-            field[(index - 1) * 6 + 5] = make_float4(J[8], J[9], J[10], J[11]);
-        }
+        // each voxel once (field_voxel, ia_device.cuh); the last voxel of a row also writes the row's zero pad
+        float4* out = reinterpret_cast<float4*>(field_voxel(field, H, W, idx_d, idx_h, idx_w));
+        out[0] = make_float4(J[0], J[1], J[2], J[3]);
+        out[1] = make_float4(J[4], J[5], J[6], J[7]);
+        out[2] = make_float4(J[8], J[9], J[10], J[11]);
         if (idx_w == W - 1) {
-            field[index * 6 + 3] = make_float4(0.f, 0.f, 0.f, 0.f);
-            field[index * 6 + 4] = make_float4(0.f, 0.f, 0.f, 0.f);
-            field[index * 6 + 5] = make_float4(0.f, 0.f, 0.f, 0.f);
+            out[3] = make_float4(0.f, 0.f, 0.f, 0.f);
+            out[4] = make_float4(0.f, 0.f, 0.f, 0.f);
+            out[5] = make_float4(0.f, 0.f, 0.f, 0.f);
         }
 #pragma unroll
         for (int i0 = 0; i0 < 3; i0++) {
@@ -1045,10 +1040,11 @@ int ia_precompute(const float* voxel_w, const float* tfs, const float* offset_k,
                   int W, float* field_out, float* voxel_d_out, float* aabb_out, ia_stream_t stream) {
     IA_REQUIRE(voxel_w && tfs && offset_k && scale_k && field_out);
     IA_REQUIRE(D > 1 && H > 1 && W > 1);
+    IA_REQUIRE((long)D * H * (W + 1) <= 0xffffffffL);  // field_voxel indexes voxels in 32 bits
     const long V = (long)D * H * W;
     if (aabb_out) aabb_init_kernel<<<1, 32, 0, (cudaStream_t)stream>>>(aabb_out);
     precompute_kernel<<<(unsigned)((V + 255) / 256), 256, 0, (cudaStream_t)stream>>>(
-        voxel_w, tfs, offset_k, scale_k, D, H, W, reinterpret_cast<float4*>(field_out), voxel_d_out, aabb_out);
+        voxel_w, tfs, offset_k, scale_k, D, H, W, field_out, voxel_d_out, aabb_out);
     IA_CHECK_CUDA(cudaPeekAtLastError());
     return IA_OK;
 }

@@ -1,9 +1,9 @@
 // ia_microbench.cu -- the measured ceiling the roofline of the gather-bound kernels is quoted against (bench.py).
 //
 // deform_query_kernel / render_fwd_kernel spend their memory time in one access shape: every lane
-// gathers its own trilinear footprint of the skinning-transform field -- 4 x-pair records of 96 bytes = 12 sectors,
-// 24 x LDG.E.128 -- from a 50 MB table, and the next address depends on the loaded data (a Broyden
-// iterate).  This kernel issues exactly that shape and nothing else (no solver arithmetic beyond the 96 FMAs that
+// gathers its own trilinear footprint of the skinning-transform field -- 4 x-pairs of 96 bytes, 24 x LDG.E.128, 3-4
+// sectors per pair -- from a 25 MB table (field_voxel, ia_device.cuh), and the next address depends on the loaded data
+// (a Broyden iterate).  This kernel issues exactly that shape and nothing else (no solver arithmetic beyond the 96 FMAs that
 // consume the loads), at the fused kernels' residency (one CTA of `warps` warps per SM, persistent), so
 //     sectors requested / time  =  what the L1 data pipe + L2 deliver for this shape on this GPU.
 // `coherent` = 1 keeps the lanes of a warp inside a 10 x 3 x 3 voxel neighbourhood as a batch of the occupancy query does
@@ -38,12 +38,10 @@ __global__ void __launch_bounds__(kWarps * 32, 1) gather_ceiling_kernel(const fl
         } else {
             x = (int)(r % (uint32_t)(W - 1)); y = (int)((r >> 8) % (uint32_t)(H - 1)); z = (int)((r >> 16) % (uint32_t)(D - 1));
         }
-        const unsigned rec[4] = {(unsigned)((z * H + y) * W + x), (unsigned)((z * H + y + 1) * W + x),
-                                 (unsigned)(((z + 1) * H + y) * W + x), (unsigned)(((z + 1) * H + y + 1) * W + x)};
         const float w0 = 0.25f + (float)(s & 15u) * 1e-3f;
 #pragma unroll
         for (int k = 0; k < 4; k++) {
-            const float* p = table + (size_t)rec[k] * kVoxelFloats;
+            const float* p = field_voxel(table, H, W, (unsigned)(z + (k >> 1)), (unsigned)(y + (k & 1)), (unsigned)x);
             const F8 A = ldg_sector(p), B = ldg_sector(p + 8), C3 = ldg_sector(p + 16);
 #pragma unroll
             for (int c = 0; c < 8; c++) acc[c] = __fmaf_rn(A.v[c], w0, acc[c]);
@@ -63,6 +61,8 @@ __global__ void __launch_bounds__(kWarps * 32, 1) gather_ceiling_kernel(const fl
 #pragma unroll
     for (int c = 0; c < 12; c++) t += acc[c];
     if (t == 123.456f && sink) sink[0] = t;
+    // nominal 12 sectors per footprint (3 per pair), the unit the kernels' field_loads counters are quoted in; a pair at
+    // odd x touches a fourth
     if (threadIdx.x == 0) atomicAdd(sectors, (unsigned long long)kWarps * 32ull * 12ull * (unsigned long long)iters);
 }
 

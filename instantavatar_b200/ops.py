@@ -14,20 +14,39 @@ from ._lib import IaNearestVertex, IaScene, IaStats, check, lib, ptr, stream
 f32 = torch.float32
 
 
+def _field_strides(H: int, W: int) -> tuple:
+    # IaScene.field: each voxel's 12 coefficients once, in rows of W + 1 voxels whose last one is zero
+    return (H * (W + 1) * 12, (W + 1) * 12, 12, 1)
+
+
 def precompute(voxel_w: torch.Tensor, tfs: torch.Tensor, offset_k: torch.Tensor, scale_k: torch.Tensor,
                want_voxel_d: bool = True):
     """precompute_cuda.precompute (deformer_torch.py:77-83).  voxel_w [1|,24,D,H,W]; tfs [1|,24,4,4].
-    Returns (field [D,H,W,24] (x-pair records), voxel_d [3,D,H,W] | None, aabb [6])."""
+    Returns (field, voxel_d [3,D,H,W] | None, aabb [6]).  field is a [D,H,W,24] view whose entry x holds the coefficients
+    of voxel x, then those of voxel x+1 (zeros at x = W-1); the storage behind it holds each voxel once (IaScene.field),
+    so consecutive x overlap.  Hand it to the kernels as it is: a copy has other strides and is refused."""
     voxel_w = voxel_w.reshape(24, *voxel_w.shape[-3:]).contiguous()
     D, H, W = voxel_w.shape[-3:]
     dev = voxel_w.device
-    fld = torch.empty((D, H, W, 24), device=dev, dtype=f32)
+    buf = torch.empty(D * H * (W + 1) * 12, device=dev, dtype=f32)
     vd = torch.empty((3, D, H, W), device=dev, dtype=f32) if want_voxel_d else None
     aabb = torch.empty(6, device=dev, dtype=f32)  # initialised by the library
     _lib.count(1); check(lib().ia_precompute(ptr(voxel_w, f32), ptr(tfs.reshape(24, 4, 4).contiguous(), f32),
                               ptr(offset_k.reshape(3).contiguous(), f32), ptr(scale_k.reshape(3).contiguous(), f32),
-                              C.c_int(D), C.c_int(H), C.c_int(W), ptr(fld), ptr(vd), ptr(aabb), stream()))
-    return fld, vd, aabb
+                              C.c_int(D), C.c_int(H), C.c_int(W), ptr(buf), ptr(vd), ptr(aabb), stream()))
+    return buf.as_strided((D, H, W, 24), _field_strides(H, W)), vd, aabb
+
+
+def _field_ptr(field: torch.Tensor) -> C.c_void_p:
+    """device address of a field returned by precompute; anything without its packed layout is refused"""
+    if not field.is_cuda:
+        raise RuntimeError("instantavatar_b200 kernels need CUDA tensors (no CPU fallback)")
+    if field.dtype != f32:
+        raise RuntimeError(f"field: expected {f32}, got {field.dtype}")
+    if field.dim() != 4 or field.shape[-1] != 24 or field.stride() != _field_strides(*field.shape[1:3]):
+        raise RuntimeError("field: expected the [D,H,W,24] view that precompute returns, strides (H*(W+1)*12, (W+1)*12, 12, 1); "
+                           f"got shape {tuple(field.shape)}, strides {field.stride()}")
+    return C.c_void_p(field.data_ptr())
 
 
 def params_to_half(enc_params: torch.Tensor, col_params: torch.Tensor, table_h=None, mlp_h=None):
@@ -189,7 +208,7 @@ def nv_nearest(nv: NearestVertex, pts):
 class Scene:
     """Per-frame read-only state (IaScene) with the tensors that keep it alive.  `nv` set: nearest-vertex deformer
     (the Fast-SNARF fields are not used)."""
-    field: torch.Tensor | None = None     # [D,H,W,24]
+    field: torch.Tensor | None = None     # [D,H,W,24] view returned by precompute
     offset_k: torch.Tensor | None = None  # [3]
     scale_k: torch.Tensor | None = None   # [3]
     tfs: torch.Tensor | None = None       # [24,4,4]
@@ -207,7 +226,7 @@ class Scene:
         s = IaScene()
         if self.field is not None:
             D, H, W, _ = self.field.shape
-            s.field = ptr(self.field, f32).value; s.D, s.H, s.W = D, H, W
+            s.field = _field_ptr(self.field).value; s.D, s.H, s.W = D, H, W
         o = lambda t: ptr(t, f32).value if t is not None else None
         s.offset_k = o(self.offset_k); s.scale_k = o(self.scale_k); s.tfs = o(self.tfs)
         s.occ_bits = ptr(self.occ_bits).value if self.occ_bits is not None else None
@@ -225,13 +244,14 @@ def gather_ceiling(field: torch.Tensor, iters: int = 200, warps: int = 12, coher
     """measured ceiling of the fused kernels' gather shape on this GPU (ia_gather_ceiling), best of `reps` timed launches
     -> {"sectors_per_s", "GBps", "ms"}"""
     D, H, W, _ = field.shape
+    fp = _field_ptr(field)
     cnt = torch.zeros(1, device=field.device, dtype=torch.int64)
     best = None
     for i in range(reps + 1):  # first launch warms L2 / instruction cache
         cnt.zero_()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        _lib.count(1); check(lib().ia_gather_ceiling(ptr(field, f32), C.c_int(D), C.c_int(H), C.c_int(W), C.c_int(iters), C.c_int(warps),
+        _lib.count(1); check(lib().ia_gather_ceiling(fp, C.c_int(D), C.c_int(H), C.c_int(W), C.c_int(iters), C.c_int(warps),
                                                      C.c_int(1 if coherent else 0), ptr(cnt), None, stream()))
         e1.record()
         e1.synchronize()
