@@ -83,10 +83,8 @@ const char* ia_last_error(void);
 /* number of SMs of the current device (grid sizing is a multiple of this) [host result] */
 int ia_sm_count(void);
 
-/* tuning knobs (do not change results): "render_rays_per_warp" in {4, 2, 1} (ray tile of ia_render_fwd*; the sharded
- * frame uses 2 and 1), "query_warps" in {12, 16} (warps per CTA of ia_deform_query without xc_best, Fast-SNARF scenes),
- * "query_lanes_per_sample" in {0 = from the load, 1, 2, 4} (lanes sharing one sample's 13 root finds in
- * ia_train_fwd_split's point query).  Any other name is IA_EINVAL ("unknown option"). */
+/* tuning knob (does not change results): "render_rays_per_warp" in {4, 2, 1} (ray tile of ia_render_fwd*; the sharded
+ * frame uses 2 and 1).  Any other name is IA_EINVAL ("unknown option"). */
 int ia_set_option(const char* name, int value);
 
 /* tiny-cuda-nn HashGrid level table (models/networks/ngp.py:27-37 config). [host] outputs. */

@@ -182,11 +182,7 @@ extern "C" int ia_image_metrics(const uint8_t* a, long frame_stride_a, long row_
     IA_REQUIRE(F <= 1 || (frame_stride_a >= (H - 1) * row_stride_a + 3L * W && frame_stride_b >= (H - 1) * row_stride_b + 3L * W));
     if (F == 0) return IA_OK;
     IA_REQUIRE(a && b && taps && sse && ssim_fx);
-    static PerDeviceFlag smem_set;
-    if (!smem_set.get()) {
-        IA_CHECK_CUDA(cudaFuncSetAttribute(image_metrics_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kMetricsSmem));
-        smem_set.set();
-    }
+    if (const int rc = allow_dynamic_smem<image_metrics_kernel>((int)kMetricsSmem)) return rc;
     MetricsArgs A;
     A.a = a; A.b = b;
     A.frame_stride_a = frame_stride_a; A.row_stride_a = row_stride_a; A.frame_stride_b = frame_stride_b; A.row_stride_b = row_stride_b;

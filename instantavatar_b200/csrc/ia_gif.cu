@@ -287,11 +287,7 @@ extern "C" int ia_gif_quantize(const uint8_t* rgba, int F, int H, int W, int swa
     IA_REQUIRE(rgba && palette && index && n_colors && workspace);
     IA_REQUIRE(workspace_bytes >= ia_gif_quantize_workspace_bytes(F));
     IA_REQUIRE(((uintptr_t)rgba & 3) == 0 && ((uintptr_t)workspace & 15) == 0);
-    static PerDeviceFlag smem_set;
-    if (!smem_set.get()) {
-        IA_CHECK_CUDA(cudaFuncSetAttribute(gif_cut_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)kCutSmem));
-        smem_set.set();
-    }
+    if (const int rc = allow_dynamic_smem<gif_cut_kernel>((int)kCutSmem)) return rc;
     const long hw = (long)H * W;
     const uchar4* px = reinterpret_cast<const uchar4*>(rgba);
     uint32_t* ws = static_cast<uint32_t*>(workspace);

@@ -46,3 +46,15 @@ struct PerDeviceFlag {
     void set() { const int d = current_device(); if (d >= 0) done[d % kMaxDevices] = true; }
 };
 
+// Opts Kernel into `bytes` of dynamic shared memory (above the default 48 KB) once per device.  The template takes the
+// kernel itself, not its type, so that kernels of one signature (render_fwd_kernel<4> and <2>) each get their own flag.
+template <auto Kernel>
+inline int allow_dynamic_smem(int bytes) {
+    static PerDeviceFlag done;
+    if (!done.get()) {
+        IA_CHECK_CUDA(cudaFuncSetAttribute(Kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, bytes));
+        done.set();
+    }
+    return IA_OK;
+}
+

@@ -11,8 +11,6 @@
 using namespace ia;
 
 static int g_render_rays = 4;  // rays per warp of the renderer (4 / 2 / 1; the sharded frame uses 2 and 1), ia_set_option
-static int g_query_warps = 12;  // warps per CTA of the point query without xc output (12 / 16), ia_set_option
-static int g_query_lanes = 0;  // lanes per point of the list-mode point query (training forward): 0 = auto, 1 / 2 / 4
 
 constexpr int kRenderWarps = 12;  // warps per CTA of the fused renderer (one CTA per SM)
 
@@ -89,6 +87,40 @@ __device__ __forceinline__ void occupied_interval(const FrameConst& fc, const in
     }
 }
 
+// A ray of the frame: origin, direction, near / far, step (raymarcher_acc.py:102) and the steps [kbeg, kend] that can
+// reach an occupied cell (empty-space skip)
+struct FrameRay {
+    float ox = 0, oy = 0, oz = 0, dx = 0, dy = 0, dz = 1, t = 0, far = 0, dt = 0;
+    int kbeg = 0, kend = -1;
+};
+
+// false (kbeg = 0, kend = -1) when no step of the ray can reach an occupied cell
+__device__ __forceinline__ bool load_ray(const RenderArgs& a, const FrameConst& fc, const int* __restrict__ cbox, int G, int ray,
+                                         FrameRay& r) {
+    r.ox = a.rays_o[ray * 3]; r.oy = a.rays_o[ray * 3 + 1]; r.oz = a.rays_o[ray * 3 + 2];
+    r.dx = a.rays_d[ray * 3]; r.dy = a.rays_d[ray * 3 + 1]; r.dz = a.rays_d[ray * 3 + 2];
+    r.t = a.near[ray]; r.far = a.far[ray];
+    r.dt = (r.far - r.t) / (float)IA_MAX_SAMPLES;
+    float t0, t1;
+    occupied_interval(fc, cbox, G, r.ox, r.oy, r.oz, r.dx, r.dy, r.dz, t0, t1);
+    if (!(cbox[6] != 0 && t0 <= t1 && r.dt > 0.f)) return false;
+    const float k0f = floorf((fmaxf(t0, r.t) - r.t) / r.dt) - 2.f, k1f = ceilf((fminf(t1, r.far) - r.t) / r.dt) + 2.f;
+    r.kbeg = (int)fminf(fmaxf(k0f, 0.f), 1024.f);
+    r.kend = (int)fminf(fmaxf(k1f, -1.f), 1024.f);
+    return true;
+}
+
+// a ray's outputs (raymarcher_acc.py:128-132): colour C + T * background (white without one), depth, alpha and the
+// number of samples marched
+__device__ __forceinline__ void store_ray(const RenderArgs& a, int ray, float Cr, float Cg, float Cb, float T, float Dp, float n) {
+    float b0 = 1.f, b1 = 1.f, b2 = 1.f;
+    if (a.bg) { b0 = a.bg[ray * 3]; b1 = a.bg[ray * 3 + 1]; b2 = a.bg[ray * 3 + 2]; }
+    const float r = Cr + T * b0, g = Cg + T * b1, b = Cb + T * b2, al = 1.0f - T;
+    a.rgb[ray * 3 + 0] = r; a.rgb[ray * 3 + 1] = g; a.rgb[ray * 3 + 2] = b;
+    a.depth[ray] = Dp; a.alpha[ray] = al; a.counter[ray] = n;
+    peer_store_rgba(a, ray, r, g, b, al);
+}
+
 // a warp's kRays rays (4 / 2 / 1) form a tile_width x (kRays / tile_width) block of pixels when the frame is tiled
 __host__ __device__ constexpr int tile_width(int rays) { return rays >= 2 ? 2 : 1; }
 
@@ -124,25 +156,14 @@ __global__ void __launch_bounds__(256) render_plan_kernel(const __grid_constant_
     if (tile < n_tiles) {
         ray = tile_ray<kRays>(tile, rl, tiled, a.image_width);
         if (ray < a.n_rays) {
-            const float ox = a.rays_o[ray * 3], oy = a.rays_o[ray * 3 + 1], oz = a.rays_o[ray * 3 + 2];
-            const float dx = a.rays_d[ray * 3], dy = a.rays_d[ray * 3 + 1], dz = a.rays_d[ray * 3 + 2];
-            float t = a.near[ray];
-            const float far = a.far[ray];
-            const float dt = (far - t) / (float)IA_MAX_SAMPLES;
-            float t0, t1;
-            occupied_interval(fc, cbox, G, ox, oy, oz, dx, dy, dz, t0, t1);
-            if (cbox[6] != 0 && t0 <= t1 && dt > 0.f) {
-                const float k0f = floorf((fmaxf(t0, t) - t) / dt) - 2.f, k1f = ceilf((fminf(t1, far) - t) / dt) + 2.f;
-                const int kbeg = (int)fminf(fmaxf(k0f, 0.f), 1024.f), kend = (int)fminf(fmaxf(k1f, -1.f), 1024.f);
-                for (int i = 0; i < kbeg; i++) t += dt;
-                for (int k = kbeg; k <= kend && t < far; k++) {
-                    const float x = __fmaf_rn(t, dx, ox), y = __fmaf_rn(t, dy, oy), z = __fmaf_rn(t, dz, oz);
-                    const int nx = (int)clampf((x - fc.occ_min[0]) * fc.occ_s[0], 0.0f, (float)G - 1.0f);
-                    const int ny = (int)clampf((y - fc.occ_min[1]) * fc.occ_s[1], 0.0f, (float)G - 1.0f);
-                    const int nz = (int)clampf((z - fc.occ_min[2]) * fc.occ_s[2], 0.0f, (float)G - 1.0f);
-                    const int bit = (nx * G + ny) * G + nz;
-                    cnt += (__ldg(occ + (bit >> 5)) >> (bit & 31)) & 1u;
-                    t += dt;
+            FrameRay r;
+            if (load_ray(a, fc, cbox, G, ray, r)) {
+                float t = r.t;
+                for (int i = 0; i < r.kbeg; i++) t += r.dt;
+                for (int k = r.kbeg; k <= r.kend && t < r.far; k++) {
+                    const float x = __fmaf_rn(t, r.dx, r.ox), y = __fmaf_rn(t, r.dy, r.oy), z = __fmaf_rn(t, r.dz, r.oz);
+                    cnt += occupied<true>(occ, fc.occ_min, fc.occ_s, G, x, y, z);
+                    t += r.dt;
                 }
             }
         } else {
@@ -154,13 +175,8 @@ __global__ void __launch_bounds__(256) render_plan_kernel(const __grid_constant_
     for (int o = 1; o < kRays; o <<= 1) tot += __shfl_xor_sync(kFull, tot, o);
     if (tile < n_tiles) {
         if (rl == 0) cost[tile] = tot;
-        if (tot == 0 && ray >= 0) {  // no sample anywhere in the tile: the fused kernel would leave T = 1, C = 0
-            float b0 = 1.f, b1 = 1.f, b2 = 1.f;
-            if (a.bg) { b0 = a.bg[ray * 3]; b1 = a.bg[ray * 3 + 1]; b2 = a.bg[ray * 3 + 2]; }
-            a.rgb[ray * 3 + 0] = 0.f + 1.f * b0; a.rgb[ray * 3 + 1] = 0.f + 1.f * b1; a.rgb[ray * 3 + 2] = 0.f + 1.f * b2;
-            a.depth[ray] = 0.f; a.alpha[ray] = 0.f; a.counter[ray] = 0.f;
-            peer_store_rgba(a, ray, 0.f + 1.f * b0, 0.f + 1.f * b1, 0.f + 1.f * b2, 0.f);
-        }
+        // no sample anywhere in the tile: the fused kernel would leave T = 1, C = 0
+        if (tot == 0 && ray >= 0) store_ray(a, ray, 0.f, 0.f, 0.f, 1.f, 0.f, 0.f);
     }
 }
 
@@ -216,26 +232,7 @@ __global__ void __launch_bounds__(kRenderWarps * 32, 1) render_fwd_kernel(const 
     RenderSmem<kNV>& sm = *reinterpret_cast<RenderSmem<kNV>*>(smem_raw);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     const int G = a.sd.s.G;
-    // ---- prologue: TMA-engine bulk copies of the occupancy bitfield and the MLP weights -------------
-    const uint32_t occ_bytes = (uint32_t)(G * G * G / 8);
-    if (threadIdx.x == 0) {
-        mbar_init(&sm.mbar, 1);
-        mbar_expect_tx(&sm.mbar, occ_bytes + kMlpHalfs * 2);
-        bulk_g2s(sm.occ, a.sd.s.occ_bits, occ_bytes, &sm.mbar);
-        bulk_g2s(sm.W, a.sd.s.mlp_h, kMlpHalfs * 2, &sm.mbar);
-    }
-    load_frame_const<kNV>(sm.fc, a.sd);
-    __syncthreads();
-    mbar_wait(&sm.mbar, 0);
-
-    EvalCtx ctx;
-    ctx.field.data = a.sd.s.field;
-    ctx.field.D = a.sd.s.D; ctx.field.H = a.sd.s.H; ctx.field.W = a.sd.s.W;
-    ctx.table = reinterpret_cast<const __half2*>(a.sd.s.table_h);
-    ctx.Wsm = sm.W;
-   
-    ctx.fc = &sm.fc;
-    ctx.hl = &a.sd.hl;
+    const EvalCtx ctx = stage_frame<kNV>(a.sd, sm.fc, sm.W, &sm.mbar, sm.occ);
     auto& ws = sm.ws[warp];
     RenderWarpExtra& wx = sm.wx[warp];
     const FrameConst& fc = sm.fc;
@@ -244,7 +241,7 @@ __global__ void __launch_bounds__(kRenderWarps * 32, 1) render_fwd_kernel(const 
     const bool tiled = a.image_width > 0 && (a.image_width % kTileW) == 0 && (a.n_rays % (a.image_width * kTileH)) == 0;
     const int n_tiles = (a.n_rays + kRays - 1) / kRays;
     const int rl = lane % kRays, jl = lane / kRays;
-    unsigned st_gather = 0, st_roots = 0, st_samples = 0, st_hit = 0, st_load = 0, st_hash = 0;
+    WorkCounters wc;
 
     for (;;) {
         int tile = 0;
@@ -256,26 +253,17 @@ __global__ void __launch_bounds__(kRenderWarps * 32, 1) render_fwd_kernel(const 
         if (tile >= n_tiles) break;
         const int ray = tile_ray<kRays>(tile, rl, tiled, a.image_width);
         const bool has = ray < a.n_rays;
-        float ox = 0, oy = 0, oz = 0, dx = 0, dy = 0, dz = 1, t = 0, far = 0, dt = 0;
-        int k = jl, kend = -1;
+        FrameRay r;
+        int k = jl;
         if (has) {
-            ox = a.rays_o[ray * 3]; oy = a.rays_o[ray * 3 + 1]; oz = a.rays_o[ray * 3 + 2];
-            dx = a.rays_d[ray * 3]; dy = a.rays_d[ray * 3 + 1]; dz = a.rays_d[ray * 3 + 2];
-            t = a.near[ray]; far = a.far[ray];
-            dt = (far - t) / (float)IA_MAX_SAMPLES;  // raymarcher_acc.py:102
             // empty-space skip: steps outside [kbeg, kend] cannot hit an occupied cell
-            float t0, t1;
-            occupied_interval(fc, cbox, G, ox, oy, oz, dx, dy, dz, t0, t1);
-            if (cbox[6] != 0 && t0 <= t1 && dt > 0.f) {
-                const float k0f = floorf((fmaxf(t0, t) - t) / dt) - 2.f, k1f = ceilf((fminf(t1, far) - t) / dt) + 2.f;
-                int kbeg = (int)fminf(fmaxf(k0f, 0.f), 1024.f);
-                kend = (int)fminf(fmaxf(k1f, -1.f), 1024.f);
-                kbeg = (kbeg / kDepth) * kDepth;
-                k = kbeg + jl;
-            }
+            if (load_ray(a, fc, cbox, G, ray, r)) k = (r.kbeg / kDepth) * kDepth + jl;
             // t_k is the k-fold sequential sum near + dt + dt + ... exactly as the reference accumulates it
-            for (int i = 0; i < k; i++) t += dt;
+            for (int i = 0; i < k; i++) r.t += r.dt;
         }
+        const float ox = r.ox, oy = r.oy, oz = r.oz, dx = r.dx, dy = r.dy, dz = r.dz, far = r.far, dt = r.dt;
+        const int kend = r.kend;
+        float t = r.t;
         float T = 1.f, Cr = 0.f, Cg = 0.f, Cb = 0.f, Dp = 0.f;  // ray state lives in lanes < kRays
         int nocc = 0;
         int qhead = 0, qcount = 0;
@@ -289,11 +277,7 @@ __global__ void __launch_bounds__(kRenderWarps * 32, 1) render_fwd_kernel(const 
                 float x = 0, y = 0, z = 0;
                 if (act) {
                     x = __fmaf_rn(t, dx, ox); y = __fmaf_rn(t, dy, oy); z = __fmaf_rn(t, dz, oz);
-                    const int nx = (int)clampf((x - fc.occ_min[0]) * fc.occ_s[0], 0.0f, (float)G - 1.0f);
-                    const int ny = (int)clampf((y - fc.occ_min[1]) * fc.occ_s[1], 0.0f, (float)G - 1.0f);
-                    const int nz = (int)clampf((z - fc.occ_min[2]) * fc.occ_s[2], 0.0f, (float)G - 1.0f);
-                    const int bit = (nx * G + ny) * G + nz;
-                    occ = (sm.occ[bit >> 5] >> (bit & 31)) & 1u;
+                    occ = occupied<false>(sm.occ, fc.occ_min, fc.occ_s, G, x, y, z);
                 }
                 const unsigned m = __ballot_sync(kFull, occ);
                 if (occ) {
@@ -321,12 +305,13 @@ __global__ void __launch_bounds__(kRenderWarps * 32, 1) render_fwd_kernel(const 
             qhead = (qhead + n) & 63;
             qcount -= n;
             if (!__any_sync(kFull, sact)) continue;
-            st_samples += sact ? 1u : 0u;
+            wc.samples += sact ? 1u : 0u;
             SampleOut so;
             if constexpr (kNV) {
-                warp_eval_nv(ctx, a.sd.nv, ws, sact, sx, sy, sz, true, lane, so, st_roots, st_hash);
+                warp_eval_nv(ctx, a.sd.nv, ws, sact, sx, sy, sz, true, lane, so, wc.net_evals, wc.hash_loads);
             } else {
-                warp_eval_samples<false>(ctx, ws, sact, sx, sy, sz, true, lane, so, st_gather, st_roots, st_load, st_hash);
+                warp_eval_samples<false>(ctx, ws, sact, sx, sy, sz, true, lane, so, wc.gathers, wc.net_evals, wc.field_loads,
+                                         wc.hash_loads);
             }
             // ---- composite in sample order (raymarcher.cu:200-235) ----
             ws.res[lane][0] = so.sigma; ws.res[lane][1] = so.r; ws.res[lane][2] = so.g; ws.res[lane][3] = so.b;
@@ -352,37 +337,11 @@ __global__ void __launch_bounds__(kRenderWarps * 32, 1) render_fwd_kernel(const 
 #pragma unroll
         for (int o = kRays; o < 32; o <<= 1) nocc += __shfl_xor_sync(kFull, nocc, o);
         if (has && jl == 0) {
-            float b0 = 1.f, b1 = 1.f, b2 = 1.f;  // raymarcher_acc.py:128-132
-            if (a.bg) { b0 = a.bg[ray * 3]; b1 = a.bg[ray * 3 + 1]; b2 = a.bg[ray * 3 + 2]; }
-            a.rgb[ray * 3 + 0] = Cr + T * b0;
-            a.rgb[ray * 3 + 1] = Cg + T * b1;
-            a.rgb[ray * 3 + 2] = Cb + T * b2;
-            a.depth[ray] = Dp;
-            a.alpha[ray] = 1.0f - T;
-            a.counter[ray] = (float)nocc;
-            peer_store_rgba(a, ray, Cr + T * b0, Cg + T * b1, Cb + T * b2, 1.0f - T);
-            st_hit += nocc > 0 ? 1u : 0u;
+            store_ray(a, ray, Cr, Cg, Cb, T, Dp, (float)nocc);
+            wc.rays_hit += nocc > 0 ? 1u : 0u;
         }
     }
-    if (a.stats) {
-#pragma unroll
-        for (int o = 16; o; o >>= 1) {
-            st_gather += __shfl_xor_sync(kFull, st_gather, o);
-            st_load += __shfl_xor_sync(kFull, st_load, o);
-            st_hash += __shfl_xor_sync(kFull, st_hash, o);
-            st_roots += __shfl_xor_sync(kFull, st_roots, o);
-            st_samples += __shfl_xor_sync(kFull, st_samples, o);
-            st_hit += __shfl_xor_sync(kFull, st_hit, o);
-        }
-        if (lane == 0) {
-            atomicAdd(&a.stats->gathers, (unsigned long long)st_gather);
-            atomicAdd(&a.stats->field_loads, (unsigned long long)st_load);
-            atomicAdd(&a.stats->hash_loads, (unsigned long long)st_hash);
-            atomicAdd(&a.stats->net_evals, (unsigned long long)st_roots);
-            atomicAdd(&a.stats->samples, (unsigned long long)st_samples);
-            atomicAdd(&a.stats->rays_hit, (unsigned long long)st_hit);
-        }
-    }
+    wc.flush(a.stats, lane);
 }
 
 // ================================================================================================
@@ -397,7 +356,6 @@ struct QueryArgs {
     // optional (split training forward, ia_train.cu): the number of points lives on the device (n = capacity)
     // and point p reads pts / writes every output at element index[p] instead of p
     const int* n_dev; const int* index;
-    int lanes_per_sample;  // point mode: 1 / 2 / 4 lanes share a point's 13 root finds (narrow batches); 0 = pick from the load
 };
 
 template <int kWarps, bool kKeepXc, bool kNV = false>
@@ -409,38 +367,23 @@ struct QuerySmem {
 };
 
 // kKeepXc: the canonical point of the winning candidate is an output (xc_best; training-time queries); queries without
-// it need 5 KB less shared memory per warp.  Fast-SNARF queries that keep it choose the lanes per point at run time
-// (a.lanes_per_sample); the others run one lane per point with a literal 1
+// it need 5 KB less shared memory per warp.  The Fast-SNARF list query (training forward) chooses the lanes per point
+// from its load; every other query runs one lane per point
 // kNV: nearest-vertex deform stage (warp_eval_nv, one lane per point)
 template <int kWarps, bool kKeepXc, bool kNV = false>
 __global__ void __launch_bounds__(kWarps * 32, 1) deform_query_kernel(const __grid_constant__ QueryArgs a) {
     extern __shared__ __align__(128) unsigned char smem_raw[];
     QuerySmem<kWarps, kKeepXc, kNV>& sm = *reinterpret_cast<QuerySmem<kWarps, kKeepXc, kNV>*>(smem_raw);
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
-    if (threadIdx.x == 0) {
-        mbar_init(&sm.mbar, 1);
-        mbar_expect_tx(&sm.mbar, kMlpHalfs * 2);
-        bulk_g2s(sm.W, a.sd.s.mlp_h, kMlpHalfs * 2, &sm.mbar);
-    }
-    load_frame_const<kNV>(sm.fc, a.sd);
-    __syncthreads();
-    mbar_wait(&sm.mbar, 0);
-    EvalCtx ctx;
-    ctx.field.data = a.sd.s.field;
-    ctx.field.D = a.sd.s.D; ctx.field.H = a.sd.s.H; ctx.field.W = a.sd.s.W;
-    ctx.table = reinterpret_cast<const __half2*>(a.sd.s.table_h);
-    ctx.Wsm = sm.W; ctx.fc = &sm.fc; ctx.hl = &a.sd.hl;
-    unsigned st_gather = 0, st_roots = 0, st_samples = 0, st_load = 0, st_hash = 0;
+    const EvalCtx ctx = stage_frame<kNV>(a.sd, sm.fc, sm.W, &sm.mbar);
+    WorkCounters wc;
     const int n_pts = a.n_dev ? min(*a.n_dev, a.n) : a.n;
     // with few points per resident warp a batch's latency (13 serial root finds per lane) is the kernel's time; k lanes per
-    // point divide it (warp_eval_samples) at no extra memory traffic.  Point mode, k = 0: about one batch per warp.
+    // point divide it (warp_eval_samples) at no extra memory traffic: about one batch per warp
     int k = 1;
-    if (kKeepXc && !kNV) {
-        k = a.lanes_per_sample;
-        if (k == 0) {
-            const int n_warps = gridDim.x * kWarps, n32 = (n_pts + 31) / 32;
-            k = 4 * n32 * 4 <= 5 * n_warps ? 4 : (4 * n32 * 2 <= 5 * n_warps ? 2 : 1);
-        }
+    if (kKeepXc && !kNV && a.n_dev) {
+        const int n_warps = gridDim.x * kWarps, n32 = (n_pts + 31) / 32;
+        k = 4 * n32 * 4 <= 5 * n_warps ? 4 : (4 * n32 * 2 <= 5 * n_warps ? 2 : 1);
     }
     const int spw = 32 / k;  // points per warp batch
     const int n_batches = (n_pts + spw - 1) / spw;
@@ -460,14 +403,16 @@ __global__ void __launch_bounds__(kWarps * 32, 1) deform_query_kernel(const __gr
         if (act) { x = a.pts[q * 3]; y = a.pts[q * 3 + 1]; z = a.pts[q * 3 + 2]; }
         SampleOut so;
         if constexpr (kNV) {
-            warp_eval_nv(ctx, a.sd.nv, sm.ws[warp], act, x, y, z, a.eval_mode != 0, lane, so, st_roots, st_hash);
+            warp_eval_nv(ctx, a.sd.nv, sm.ws[warp], act, x, y, z, a.eval_mode != 0, lane, so, wc.net_evals, wc.hash_loads);
         } else if constexpr (kKeepXc) {
-            warp_eval_samples<kKeepXc>(ctx, sm.ws[warp], act, x, y, z, a.eval_mode != 0, lane, so, st_gather, st_roots, st_load, st_hash, k);
+            warp_eval_samples<kKeepXc>(ctx, sm.ws[warp], act, x, y, z, a.eval_mode != 0, lane, so, wc.gathers, wc.net_evals,
+                                       wc.field_loads, wc.hash_loads, k);
         } else {
-            warp_eval_samples<kKeepXc>(ctx, sm.ws[warp], act, x, y, z, a.eval_mode != 0, lane, so, st_gather, st_roots, st_load, st_hash);
+            warp_eval_samples<kKeepXc>(ctx, sm.ws[warp], act, x, y, z, a.eval_mode != 0, lane, so, wc.gathers, wc.net_evals,
+                                       wc.field_loads, wc.hash_loads);
         }
         act = act && owner;
-        st_samples += act ? 1u : 0u;
+        wc.samples += act ? 1u : 0u;
         if (act) {
             a.sigma[q] = so.sigma;
             a.rgb[q * 3] = so.r; a.rgb[q * 3 + 1] = so.g; a.rgb[q * 3 + 2] = so.b;
@@ -477,23 +422,7 @@ __global__ void __launch_bounds__(kWarps * 32, 1) deform_query_kernel(const __gr
             if (a.best_init) a.best_init[q] = (int8_t)so.best;
         }
     }
-    if (a.stats) {
-#pragma unroll
-        for (int o = 16; o; o >>= 1) {
-            st_gather += __shfl_xor_sync(kFull, st_gather, o);
-            st_load += __shfl_xor_sync(kFull, st_load, o);
-            st_hash += __shfl_xor_sync(kFull, st_hash, o);
-            st_roots += __shfl_xor_sync(kFull, st_roots, o);
-            st_samples += __shfl_xor_sync(kFull, st_samples, o);
-        }
-        if (lane == 0) {
-            atomicAdd(&a.stats->gathers, (unsigned long long)st_gather);
-            atomicAdd(&a.stats->field_loads, (unsigned long long)st_load);
-            atomicAdd(&a.stats->hash_loads, (unsigned long long)st_hash);
-            atomicAdd(&a.stats->net_evals, (unsigned long long)st_roots);
-            atomicAdd(&a.stats->samples, (unsigned long long)st_samples);
-        }
-    }
+    wc.flush(a.stats, lane);
 }
 
 // ================================================================================================
@@ -544,7 +473,7 @@ __global__ void __launch_bounds__(kOccRootWarps * 32, kOccRootCtas) occupancy_ro
     const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
     FieldDesc field;
     field.data = a.sd.s.field; field.D = a.sd.s.D; field.H = a.sd.s.H; field.W = a.sd.s.W;
-    unsigned st_gather = 0, st_roots = 0, st_samples = 0, st_load = 0;
+    WorkCounters wc;
     // the grid is persistent, so a warp's slot is its own for the whole launch
     float (*cand)[kNumInit][32] =
         reinterpret_cast<float (*)[kNumInit][32]>(a.cand + (size_t)(blockIdx.x * kOccRootWarps + warp) * 3 * kNumInit * 32);
@@ -570,7 +499,7 @@ __global__ void __launch_bounds__(kOccRootWarps * 32, kOccRootCtas) occupancy_ro
             y = ((float)cj / fG + jit[1] / fG) * (a.grid_aabb[4] - a.grid_aabb[1]) + a.grid_aabb[1];
             z = ((float)ck / fG + jit[2] / fG) * (a.grid_aabb[5] - a.grid_aabb[2]) + a.grid_aabb[2];
         }
-        st_samples += act ? 1u : 0u;
+        wc.samples += act ? 1u : 0u;
         unsigned kept = 0;
         float xc[3] = {0.f, 0.f, 0.f};
         if constexpr (kNV) {
@@ -580,14 +509,14 @@ __global__ void __launch_bounds__(kOccRootWarps * 32, kOccRootCtas) occupancy_ro
                 if (v >= 0) { nv_apply(a.sd.nv, v, x, y, z, xc); kept = 1u; }
             }
         } else {
-            kept = warp_find_roots<false>(field, fc, cand, act, x, y, z, lane, st_gather, st_load);
+            kept = warp_find_roots<false>(field, fc, cand, act, x, y, z, lane, wc.gathers, wc.field_loads);
         }
         int total;
         int pos = warp_excl_scan(__popc(kept), lane, total);
         int base = 0;
         if (lane == 0 && total) base = atomicAdd(&a.counters[1], total);
         pos += __shfl_sync(kFull, base, 0);
-        st_roots += __popc(kept);
+        wc.net_evals += __popc(kept);
         for (unsigned m = kept; m; m &= m - 1) {
             const int b = __ffs(m) - 1;
             OccRoot r;
@@ -598,21 +527,7 @@ __global__ void __launch_bounds__(kOccRootWarps * 32, kOccRootCtas) occupancy_ro
         }
         __syncwarp();
     }
-    if (a.stats) {
-#pragma unroll
-        for (int o = 16; o; o >>= 1) {
-            st_gather += __shfl_xor_sync(kFull, st_gather, o);
-            st_load += __shfl_xor_sync(kFull, st_load, o);
-            st_roots += __shfl_xor_sync(kFull, st_roots, o);
-            st_samples += __shfl_xor_sync(kFull, st_samples, o);
-        }
-        if (lane == 0) {
-            atomicAdd(&a.stats->gathers, (unsigned long long)st_gather);
-            atomicAdd(&a.stats->field_loads, (unsigned long long)st_load);
-            atomicAdd(&a.stats->net_evals, (unsigned long long)st_roots);
-            atomicAdd(&a.stats->samples, (unsigned long long)st_samples);
-        }
-    }
+    wc.flush(a.stats, lane);
 }
 
 // Kernel B: 32 roots per warp -> hash encoding -> density net (mlp_density_tile16, the first half of mlp_tile16: the same
@@ -632,24 +547,16 @@ __global__ void __launch_bounds__(kOccNetWarps * 32, kOccNetCtas) occupancy_net_
     const __half2* table = reinterpret_cast<const __half2*>(a.sd.s.table_h);
     const int n = a.counters[1];
     const int g = lane >> 2, t = lane & 3;
-    unsigned st_hash = 0;
+    WorkCounters wc;
     for (int base = (blockIdx.x * kOccNetWarps + warp) * 32; base < n; base += gridDim.x * kOccNetWarps * 32) {
         const int r = base + lane;
         int cell = -1;
-        __half2* arow = reinterpret_cast<__half2*>(&At[warp][lane][0]);
-        if (r < n) {
+        float nrm[3];
+        feature_row(reinterpret_cast<__half2*>(&At[warp][lane][0]), table, a.sd.hl, cs, cs + 3, r < n, [&](float x[3]) {
             const float4 v = reinterpret_cast<const float4*>(a.roots)[r];
             cell = __float_as_int(v.w);
-            // ngp.py:75,77: x = (x - center) / scale + 0.5 ; clamp [0,1]
-            const float n0 = fminf(fmaxf((v.x - cs[0]) / cs[3] + 0.5f, 0.f), 1.f);
-            const float n1 = fminf(fmaxf((v.y - cs[1]) / cs[4] + 0.5f, 0.f), 1.f);
-            const float n2 = fminf(fmaxf((v.z - cs[2]) / cs[5] + 0.5f, 0.f), 1.f);
-#pragma unroll 4
-            for (int l = 0; l < kLevels; l++) arow[l] = hash_encode_level(table, a.sd.hl, l, n0, n1, n2, &st_hash);
-        } else {
-#pragma unroll
-            for (int l = 0; l < kLevels; l++) arow[l] = __floats2half2_rn(0.f, 0.f);
-        }
+            x[0] = v.x; x[1] = v.y; x[2] = v.z;
+        }, nrm, &wc.hash_loads);
         __syncwarp();
 #pragma unroll
         for (int mt = 0; mt < 2; mt++) {
@@ -677,11 +584,7 @@ __global__ void __launch_bounds__(kOccNetWarps * 32, kOccNetCtas) occupancy_net_
         }
         __syncwarp();
     }
-    if (a.stats) {
-#pragma unroll
-        for (int o = 16; o; o >>= 1) st_hash += __shfl_xor_sync(kFull, st_hash, o);
-        if (lane == 0) atomicAdd(&a.stats->hash_loads, (unsigned long long)st_hash);
-    }
+    wc.flush(a.stats, lane);
 }
 
 // ================================================================================================
@@ -744,16 +647,9 @@ __global__ void __launch_bounds__(kWarps * 32) ngp_forward_kernel(const __grid_c
     for (int bidx = blockIdx.x * kWarps + warp; bidx < n_batches; bidx += gridDim.x * kWarps) {
         const int p = bidx * 32 + lane;
         const bool has = p < n;
-        __half2* arow = reinterpret_cast<__half2*>(&At[warp][lane][0]);
-        if (has) {
-            const float n0 = fminf(fmaxf((x[p * 3] - cs[0]) / cs[3] + 0.5f, 0.f), 1.f);
-            const float n1 = fminf(fmaxf((x[p * 3 + 1] - cs[1]) / cs[4] + 0.5f, 0.f), 1.f);
-            const float n2 = fminf(fmaxf((x[p * 3 + 2] - cs[2]) / cs[5] + 0.5f, 0.f), 1.f);
-#pragma unroll 4
-            for (int l = 0; l < kLevels; l++) arow[l] = hash_encode_level(table, sd.hl, l, n0, n1, n2);
-        } else {
-            for (int l = 0; l < kLevels; l++) arow[l] = __floats2half2_rn(0.f, 0.f);
-        }
+        float nrm[3];
+        feature_row(reinterpret_cast<__half2*>(&At[warp][lane][0]), table, sd.hl, cs, cs + 3, has,
+                    [&](float xp[3]) { xp[0] = x[p * 3]; xp[1] = x[p * 3 + 1]; xp[2] = x[p * 3 + 2]; }, nrm);
         __syncwarp();
         mlp_tile16(&At[warp][0][0], W, &res[warp][0], lane);
         mlp_tile16(&At[warp][16][0], W, &res[warp][16], lane);
@@ -786,12 +682,11 @@ __global__ void __launch_bounds__(kWarps * 32) tcnn_encoder_forward_kernel(const
     for (int bidx = blockIdx.x * kWarps + warp; bidx < n_batches; bidx += gridDim.x * kWarps) {
         const int p = bidx * 32 + lane;
         __half2* arow = reinterpret_cast<__half2*>(&At[warp][lane][0]);
-        if (p < n) {
-            const float n0 = fminf(fmaxf(x[p * 3], 0.f), 1.f), n1 = fminf(fmaxf(x[p * 3 + 1], 0.f), 1.f), n2 = fminf(fmaxf(x[p * 3 + 2], 0.f), 1.f);
-#pragma unroll 4
-            for (int l = 0; l < kLevels; l++) arow[l] = hash_encode_level(table, sd.hl, l, n0, n1, n2);
+        if (p < n) {  // the shim's inputs are in [0,1]^3 already: clamped only
+            encode_row(arow, table, sd.hl, fminf(fmaxf(x[p * 3], 0.f), 1.f), fminf(fmaxf(x[p * 3 + 1], 0.f), 1.f),
+                       fminf(fmaxf(x[p * 3 + 2], 0.f), 1.f));
         } else {
-            for (int l = 0; l < kLevels; l++) arow[l] = __floats2half2_rn(0.f, 0.f);
+            zero_row(arow);
         }
         __syncwarp();
 #pragma unroll
@@ -1008,16 +903,6 @@ int ia_set_option(const char* name, int value) {
         g_render_rays = value;
         return IA_OK;
     }
-    if (!strcmp(name, "query_warps")) {
-        IA_REQUIRE(value == 12 || value == 16);
-        g_query_warps = value;
-        return IA_OK;
-    }
-    if (!strcmp(name, "query_lanes_per_sample")) {
-        IA_REQUIRE(value == 0 || value == 1 || value == 2 || value == 4);
-        g_query_lanes = value;
-        return IA_OK;
-    }
     return set_err(IA_EINVAL, "unknown option: %s", name);
 }
 
@@ -1092,11 +977,7 @@ size_t ia_render_workspace_bytes(int n_rays) { return 256 + 2 * sizeof(int) * (s
 template <int kRays, bool kNV = false>
 static int launch_render(RenderArgs& a, bool plan, int* ws_cost, int* ws_order, cudaStream_t st) {
     const size_t smem = sizeof(RenderSmem<kNV>);
-    static PerDeviceFlag attr_set;
-    if (!attr_set.get()) {
-        IA_CHECK_CUDA(cudaFuncSetAttribute(render_fwd_kernel<kRays, kNV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_set.set();
-    }
+    if (const int rc = allow_dynamic_smem<render_fwd_kernel<kRays, kNV>>((int)smem)) return rc;
     const int n_tiles = (a.n_rays + kRays - 1) / kRays;
     int grid = sm_count();
     if (grid <= 0) return set_err(IA_ECUDA, "no CUDA device%s");
@@ -1115,11 +996,7 @@ static int launch_render(RenderArgs& a, bool plan, int* ws_cost, int* ws_order, 
 template <int kWarps, bool kKeepXc, bool kNV = false>
 static int launch_query_t(QueryArgs& a, cudaStream_t stream) {
     const size_t smem = sizeof(QuerySmem<kWarps, kKeepXc, kNV>);
-    static PerDeviceFlag attr_set;
-    if (!attr_set.get()) {
-        IA_CHECK_CUDA(cudaFuncSetAttribute(deform_query_kernel<kWarps, kKeepXc, kNV>, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_set.set();
-    }
+    if (const int rc = allow_dynamic_smem<deform_query_kernel<kWarps, kKeepXc, kNV>>((int)smem)) return rc;
     const int n_batches = (a.n + 31) / 32;
     int grid = sm_count();
     if (grid <= 0) return set_err(IA_ECUDA, "no CUDA device%s");
@@ -1131,12 +1008,10 @@ static int launch_query_t(QueryArgs& a, cudaStream_t stream) {
 
 static int launch_query(QueryArgs& a, cudaStream_t stream) {
     if (a.sd.s.nv) {  // nearest-vertex deformer: one lane per point
-        a.lanes_per_sample = 1;
         if (a.xc_best) return launch_query_t<12, true, true>(a, stream);
         return launch_query_t<12, false, true>(a, stream);
     }
     if (a.xc_best) return launch_query_t<12, true>(a, stream);
-    if (g_query_warps == 16) return launch_query_t<16, false>(a, stream);
     return launch_query_t<12, false>(a, stream);
 }
 
@@ -1210,7 +1085,7 @@ int ia_deform_query(const IaScene* scene, const float* pts, int n, int eval_mode
     a.pts = pts; a.n = n; a.eval_mode = eval_mode; a.rgb = rgb; a.sigma = sigma; a.xc_best = xc_best;
     a.best_init = best_init; a.stats = stats;
     a.batch_counter = nullptr;
-    a.n_dev = nullptr; a.index = nullptr; a.lanes_per_sample = 1;
+    a.n_dev = nullptr; a.index = nullptr;
     return launch_query(a, (cudaStream_t)stream);
 }
 
@@ -1228,7 +1103,7 @@ __attribute__((visibility("hidden"))) int ia_internal_query_list(const IaScene* 
     a.pts = pts; a.n = capacity; a.eval_mode = eval_mode; a.rgb = rgb; a.sigma = sigma; a.xc_best = xc_best;
     a.best_init = best_init; a.stats = stats;
     a.batch_counter = batch_counter;
-    a.n_dev = n_dev; a.index = index; a.lanes_per_sample = g_query_lanes;
+    a.n_dev = n_dev; a.index = index;
     return launch_query(a, (cudaStream_t)stream);
 }
 

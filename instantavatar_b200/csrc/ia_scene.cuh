@@ -70,6 +70,29 @@ __device__ __forceinline__ void load_frame_const(FrameConst& fc, const SceneDev&
     }
 }
 
+// Prologue of the frame kernels that stage the frame in shared memory: TMA-engine bulk copies of the occupancy bits
+// (when occ is given) and the MLP weights, the frame constants, then the evaluation context of the CTA's warps
+template <bool kNV>
+__device__ __forceinline__ EvalCtx stage_frame(const SceneDev& sd, FrameConst& fc, __half* W, uint64_t* mbar,
+                                               uint32_t* occ = nullptr) {
+    const uint32_t occ_bytes = occ ? (uint32_t)(sd.s.G * sd.s.G * sd.s.G / 8) : 0u;
+    if (threadIdx.x == 0) {
+        mbar_init(mbar, 1);
+        mbar_expect_tx(mbar, occ_bytes + kMlpHalfs * 2);
+        if (occ) bulk_g2s(occ, sd.s.occ_bits, occ_bytes, mbar);
+        bulk_g2s(W, sd.s.mlp_h, kMlpHalfs * 2, mbar);
+    }
+    load_frame_const<kNV>(fc, sd);
+    __syncthreads();
+    mbar_wait(mbar, 0);
+    EvalCtx ctx;
+    ctx.field.data = sd.s.field;
+    ctx.field.D = sd.s.D; ctx.field.H = sd.s.H; ctx.field.W = sd.s.W;
+    ctx.table = reinterpret_cast<const __half2*>(sd.s.table_h);
+    ctx.Wsm = W; ctx.fc = &fc; ctx.hl = &sd.hl;
+    return ctx;
+}
+
 
 int ia_nv_check(const IaNearestVertex* nv);  // ia_nearest.cu
 

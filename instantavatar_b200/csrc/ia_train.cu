@@ -65,11 +65,7 @@ __global__ void __launch_bounds__(256) train_march_kernel(TrainMarchArgs a) {
         bool occ = false;
         if (act) {  // occupancy test on the un-jittered position, raymarcher.cu:140-152
             const float x = __fmaf_rn(t, dx, ox), y = __fmaf_rn(t, dy, oy), z = __fmaf_rn(t, dz, oz);
-            const int nx = (int)clampf((x - occ_min[0]) * occ_s[0], 0.0f, (float)G - 1.0f);
-            const int ny = (int)clampf((y - occ_min[1]) * occ_s[1], 0.0f, (float)G - 1.0f);
-            const int nz = (int)clampf((z - occ_min[2]) * occ_s[2], 0.0f, (float)G - 1.0f);
-            const int bit = (nx * G + ny) * G + nz;
-            occ = (__ldg(a.occ_bits + (bit >> 5)) >> (bit & 31)) & 1u;
+            occ = occupied<true>(a.occ_bits, occ_min, occ_s, G, x, y, z);
         }
         const unsigned m = __ballot_sync(kFull, occ);
         const int slot_s = ray_count + __popc(m & ((1u << lane) - 1u));
@@ -490,19 +486,12 @@ __global__ void __launch_bounds__(kBwdWarps * 32, 1) ngp_backward_kernel(const _
         const int p = tile * 32 + lane;
         const bool has = p < count;
         const int nrows = min(32, count - tile * 32);
-        float n0 = 0, n1 = 0, n2 = 0, dsig = 0, dr = 0, dg = 0, db = 0;
-        __half2* arow = reinterpret_cast<__half2*>(&ws.At[lane][0]);
-        if (has) {
-            n0 = fminf(fmaxf((a.xc[p * 3] - sm.cs[0]) / sm.cs[3] + 0.5f, 0.f), 1.f);
-            n1 = fminf(fmaxf((a.xc[p * 3 + 1] - sm.cs[1]) / sm.cs[4] + 0.5f, 0.f), 1.f);
-            n2 = fminf(fmaxf((a.xc[p * 3 + 2] - sm.cs[2]) / sm.cs[5] + 0.5f, 0.f), 1.f);
+        float dsig = 0, dr = 0, dg = 0, db = 0, nrm[3];
+        feature_row(reinterpret_cast<__half2*>(&ws.At[lane][0]), table, a.sd.hl, sm.cs, sm.cs + 3, has, [&](float x[3]) {
+            x[0] = a.xc[p * 3]; x[1] = a.xc[p * 3 + 1]; x[2] = a.xc[p * 3 + 2];
             dsig = a.dsigma[p]; dr = a.drgb[p * 3]; dg = a.drgb[p * 3 + 1]; db = a.drgb[p * 3 + 2];
-#pragma unroll 4
-            for (int l = 0; l < kLevels; l++) arow[l] = hash_encode_level(table, a.sd.hl, l, n0, n1, n2);
-        } else {
-#pragma unroll
-            for (int l = 0; l < kLevels; l++) arow[l] = __floats2half2_rn(0.f, 0.f);
-        }
+        }, nrm);
+        const float n0 = nrm[0], n1 = nrm[1], n2 = nrm[2];
         __syncwarp();
         mlp_bwd_tile16(&ws.At[0][0], sm.W, lane, 0, dsig, dr, dg, db, a.grad_scale, a.scratch, (long)tile * 32, nrows, ws.dEnc);
         mlp_bwd_tile16(&ws.At[16][0], sm.W, lane, 1, dsig, dr, dg, db, a.grad_scale, a.scratch, (long)tile * 32, nrows, ws.dEnc);
@@ -730,13 +719,11 @@ __global__ void __launch_bounds__(kBwdWarps * 32, 1) tcnn_encoder_backward_kerne
         const bool has = p < a.n;
         float n0 = 0, n1 = 0, n2 = 0;
         __half2* arow = reinterpret_cast<__half2*>(&ws.At[lane][0]);
-        if (has) {
+        if (has) {  // the shim's inputs are in [0,1]^3 already: clamped only
             n0 = fminf(fmaxf(a.x[p * 3], 0.f), 1.f); n1 = fminf(fmaxf(a.x[p * 3 + 1], 0.f), 1.f); n2 = fminf(fmaxf(a.x[p * 3 + 2], 0.f), 1.f);
-#pragma unroll 4
-            for (int l = 0; l < kLevels; l++) arow[l] = hash_encode_level(table, a.sd.hl, l, n0, n1, n2);
+            encode_row(arow, table, a.sd.hl, n0, n1, n2);
         } else {
-#pragma unroll
-            for (int l = 0; l < kLevels; l++) arow[l] = __floats2half2_rn(0.f, 0.f);
+            zero_row(arow);
         }
         __syncwarp();
         enc_bwd_tile16(&ws.At[0][0], sm.W, lane, 0, a.dout16, a.n, a.grad_scale, a.scratch, (long)tile * 32, ws.dEnc);
@@ -1441,11 +1428,7 @@ int ia_ngp_backward(const IaScene* scene, const float* xc, const float* dsigma, 
     a.grad_enc = grad_enc; a.scratch = reinterpret_cast<__half*>(scratch); a.denc_out = denc_out;
     cudaStream_t st = (cudaStream_t)stream;
     const size_t smem = sizeof(BwdSmem);
-    static PerDeviceFlag attr_set;
-    if (!attr_set.get()) {
-        IA_CHECK_CUDA(cudaFuncSetAttribute(ngp_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_set.set();
-    }
+    if (const int rc = allow_dynamic_smem<ngp_backward_kernel>((int)smem)) return rc;
     const int sms = sm_count();
     if (sms <= 0) return set_err(IA_ECUDA, "no CUDA device%s");
     const int n_tiles = (capacity + 31) / 32;
@@ -1470,11 +1453,7 @@ int ia_tcnn_encoder_backward(const IaScene* scene, const float* x01, const float
     a.scratch = reinterpret_cast<__half*>(scratch); a.denc_out = denc_out;
     cudaStream_t st = (cudaStream_t)stream;
     const size_t smem = sizeof(BwdSmem);
-    static PerDeviceFlag attr_set;
-    if (!attr_set.get()) {
-        IA_CHECK_CUDA(cudaFuncSetAttribute(tcnn_encoder_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_set.set();
-    }
+    if (const int rc = allow_dynamic_smem<tcnn_encoder_backward_kernel>((int)smem)) return rc;
     const int sms = sm_count();
     if (sms <= 0) return set_err(IA_ECUDA, "no CUDA device%s");
     IA_CHECK_CUDA(cudaMemsetAsync(scratch, 0, (size_t)((n + 31) / 32 * 32) * kRowHalfs * sizeof(__half), st));
@@ -1500,11 +1479,7 @@ int ia_tcnn_mlp_backward(const void* mlp_h, const float* in15, const float* dout
     a.scratch = reinterpret_cast<__half*>(scratch); a.din15 = din15;
     cudaStream_t st = (cudaStream_t)stream;
     const size_t smem = (size_t)kMlpAllHalfs * sizeof(__half);
-    static PerDeviceFlag attr_set;
-    if (!attr_set.get()) {
-        IA_CHECK_CUDA(cudaFuncSetAttribute(tcnn_mlp_backward_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, (int)smem));
-        attr_set.set();
-    }
+    if (const int rc = allow_dynamic_smem<tcnn_mlp_backward_kernel>((int)smem)) return rc;
     const int sms = sm_count();
     if (sms <= 0) return set_err(IA_ECUDA, "no CUDA device%s");
     IA_CHECK_CUDA(cudaMemsetAsync(scratch, 0, (size_t)((n + 31) / 32 * 32) * kRowHalfs * sizeof(__half), st));

@@ -140,11 +140,7 @@ extern "C" int ia_knn1(const float* pts, int n, const float* verts, int n_verts,
     if (n == 0) return IA_OK;
     IA_REQUIRE(pts && verts && idx_out && dist2_out);
     const size_t smem = (size_t)(n_verts < kVertTile ? n_verts : kVertTile) * 3 * sizeof(float);
-    static PerDeviceFlag attr_set;
-    if (!attr_set.get()) {
-        IA_CHECK_CUDA(cudaFuncSetAttribute(knn1_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kVertTile * 3 * (int)sizeof(float)));
-        attr_set.set();
-    }
+    if (const int rc = allow_dynamic_smem<knn1_kernel>(kVertTile * 3 * (int)sizeof(float))) return rc;
     knn1_kernel<<<(n + 255) / 256, 256, smem, (cudaStream_t)stream>>>(pts, n, verts, n_verts, idx_out, dist2_out);
     IA_CHECK_CUDA(cudaPeekAtLastError());
     return IA_OK;
@@ -166,11 +162,7 @@ extern "C" int ia_voxelize_weights(const float* verts, const float* vert_weights
     // the pass count decides which buffer the blend is written to, so that the last pass lands in lbs_voxel
     a.out = (smooth_passes & 1) ? scratch : lbs_voxel;
     const size_t smem = (size_t)(n_verts < kVertTile ? n_verts : kVertTile) * 3 * sizeof(float);
-    static PerDeviceFlag attr_set;
-    if (!attr_set.get()) {
-        IA_CHECK_CUDA(cudaFuncSetAttribute(knn_blend_kernel, cudaFuncAttributeMaxDynamicSharedMemorySize, kVertTile * 3 * (int)sizeof(float)));
-        attr_set.set();
-    }
+    if (const int rc = allow_dynamic_smem<knn_blend_kernel>(kVertTile * 3 * (int)sizeof(float))) return rc;
     knn_blend_kernel<<<blocks, 256, smem, st>>>(a);
     IA_CHECK_CUDA(cudaPeekAtLastError());
     float* src = a.out;

@@ -138,21 +138,13 @@ __device__ __forceinline__ void warp_eval_samples(const EvalCtx& ctx, WarpScratc
         const int r = base + lane;
         const bool has = r < total;
         int sl = 0, sb = 0;
-        __half2* arow = reinterpret_cast<__half2*>(&ws.At[lane][0]);
-        if (has) {
-            const int src = ws.roots[r];
-            sl = src & 31; sb = src >> 5;
-            const float x0 = ws.cand[0][sb][sl], x1 = ws.cand[1][sb][sl], x2 = ws.cand[2][sb][sl];
-            // ngp.py:75,77: x = (x - center) / scale + 0.5 ; clamp [0,1]
-            const float n0 = fminf(fmaxf((x0 - fc.net_center[0]) / fc.net_scale[0] + 0.5f, 0.f), 1.f);
-            const float n1 = fminf(fmaxf((x1 - fc.net_center[1]) / fc.net_scale[1] + 0.5f, 0.f), 1.f);
-            const float n2 = fminf(fmaxf((x2 - fc.net_center[2]) / fc.net_scale[2] + 0.5f, 0.f), 1.f);
-#pragma unroll 4
-            for (int l = 0; l < kLevels; l++) arow[l] = hash_encode_level(ctx.table, *ctx.hl, l, n0, n1, n2, &nhash);
-        } else {
-#pragma unroll
-            for (int l = 0; l < kLevels; l++) arow[l] = __floats2half2_rn(0.f, 0.f);
-        }
+        float nrm[3];
+        feature_row(reinterpret_cast<__half2*>(&ws.At[lane][0]), ctx.table, *ctx.hl, fc.net_center, fc.net_scale, has,
+                    [&](float x[3]) {
+                        const int src = ws.roots[r];
+                        sl = src & 31; sb = src >> 5;
+                        x[0] = ws.cand[0][sb][sl]; x[1] = ws.cand[1][sb][sl]; x[2] = ws.cand[2][sb][sl];
+                    }, nrm, &nhash);
         __syncwarp();
         mlp_tile16(&ws.At[0][0], ctx.Wsm, &ws.res[0], lane);
         if (total - base > 16) mlp_tile16(&ws.At[16][0], ctx.Wsm, &ws.res[16], lane);
@@ -229,18 +221,9 @@ __device__ __forceinline__ void warp_eval_nv(const EvalCtx& ctx, const NvDev& nv
     __syncwarp();
     if (total > 0) {
         const bool has = lane < total;
-        __half2* arow = reinterpret_cast<__half2*>(&ws.At[lane][0]);
-        if (has) {
-            // ngp.py:75,77: x = (x - center) / scale + 0.5 ; clamp [0,1]
-            const float n0 = fminf(fmaxf((ws.cx[0][lane] - fc.net_center[0]) / fc.net_scale[0] + 0.5f, 0.f), 1.f);
-            const float n1 = fminf(fmaxf((ws.cx[1][lane] - fc.net_center[1]) / fc.net_scale[1] + 0.5f, 0.f), 1.f);
-            const float n2 = fminf(fmaxf((ws.cx[2][lane] - fc.net_center[2]) / fc.net_scale[2] + 0.5f, 0.f), 1.f);
-#pragma unroll 4
-            for (int l = 0; l < kLevels; l++) arow[l] = hash_encode_level(ctx.table, *ctx.hl, l, n0, n1, n2, &nhash);
-        } else {
-#pragma unroll
-            for (int l = 0; l < kLevels; l++) arow[l] = __floats2half2_rn(0.f, 0.f);
-        }
+        float nrm[3];
+        feature_row(reinterpret_cast<__half2*>(&ws.At[lane][0]), ctx.table, *ctx.hl, fc.net_center, fc.net_scale, has,
+                    [&](float x[3]) { x[0] = ws.cx[0][lane]; x[1] = ws.cx[1][lane]; x[2] = ws.cx[2][lane]; }, nrm, &nhash);
         __syncwarp();
         mlp_tile16(&ws.At[0][0], ctx.Wsm, &ws.res[0], lane);
         if (total > 16) mlp_tile16(&ws.At[16][0], ctx.Wsm, &ws.res[16], lane);

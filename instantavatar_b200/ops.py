@@ -263,11 +263,13 @@ def gather_ceiling(field: torch.Tensor, iters: int = 200, warps: int = 12, coher
 
 
 # the library's tuning knobs (ia_set_option) and their defaults, mirrored here so that a caller can change one temporarily
-_OPTIONS = {"render_rays_per_warp": 4, "query_warps": 12, "query_lanes_per_sample": 0}
+_OPTIONS = {"render_rays_per_warp": 4}
 # retired options, still readable (bench.py reports and sets them) at the one value the kernels have: the three-launch
-# training forward (train_split) with one warp per ray (train_rays_per_warp), and 12 warps per CTA in the fused renderer
-# (render_warps)
-_FIXED_OPTIONS = {"train_split": 1, "train_rays_per_warp": 1, "render_warps": 12}
+# training forward (train_split) with one warp per ray (train_rays_per_warp), 12 warps per CTA in the fused renderer
+# (render_warps) and the point query (query_warps), and the list query's lanes per sample picked from its load
+# (query_lanes_per_sample = 0)
+_FIXED_OPTIONS = {"train_split": 1, "train_rays_per_warp": 1, "render_warps": 12, "query_warps": 12,
+                  "query_lanes_per_sample": 0}
 _train_ws: dict = {}
 
 

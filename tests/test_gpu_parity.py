@@ -252,9 +252,8 @@ def test_render_every_ray_tile_agrees(sc, dev):
             np.testing.assert_array_equal(o2[k], outs[0][k])
 
 
-def test_occupancy_query_shards_reproduce_the_grid(sc, dev):
-    """strided shards of ia_occupancy_query max-reduce to the bits of the single launch; so
-    does the 16-warp launch"""
+def test_occupancy_query_strided_shards_reproduce_the_grid(sc, dev):
+    """strided shards of ia_occupancy_query max-reduce to the bits of the single launch"""
     import torch
     from instantavatar_b200 import ops
     scene, _ = dev
@@ -268,8 +267,3 @@ def test_occupancy_query_shards_reproduce_the_grid(sc, dev):
         for r in range(n_shards):
             acc = torch.maximum(acc, ops.occupancy_query(scene, jit, aabb, shard=(r, n_shards)))
         assert torch.equal(acc, full), n_shards
-    try:   # the 16-warp launch shape
-        ops.set_option("query_warps", 16)
-        assert torch.equal(ops.occupancy_query(scene, jit, aabb), full)
-    finally:
-        ops.set_option("query_warps", 12)

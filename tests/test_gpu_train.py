@@ -96,35 +96,58 @@ def test_train_fwd_matches_oracle(sc, dev):
     assert (ref["alpha"] > 0.5).sum() > 100
 
 
-def test_train_fwd_matches_golden_bit_for_bit(sc, dev):
-    """The training forward at every lanes-per-sample setting of its point query equals the others and the stored
-    result of the retired one-kernel form (oracle/train_fwd_golden.py) in every output, every live saved-for-backward
-    value and its stats; and every live sample equals the point query at the posed point the march placed it at"""
+def _list_query_lanes(n_rays, n_samples):
+    """lanes per sample of the training forward's list query (deform_query_kernel's rule): the grid of launch_query_t<12>
+    over a capacity of n_rays * IA_MAX_SAMPLES points, then 4, 2 or 1 lanes as n_samples leave about one batch per warp"""
+    from instantavatar_b200 import _lib
+    warps = 12
+    grid = min(_lib.lib().ia_sm_count(), ((n_rays * _lib.IA_MAX_SAMPLES + 31) // 32 + warps - 1) // warps)
+    n_warps, n32 = grid * warps, (n_samples + 31) // 32
+    return 4 if 16 * n32 <= 5 * n_warps else (2 if 8 * n32 <= 5 * n_warps else 1)
+
+
+def test_train_fwd_matches_golden_at_every_list_lane_count(sc, dev):
+    """The training forward equals the stored result of the retired one-kernel form (oracle/train_fwd_golden.py) in every
+    output, every live saved-for-backward value and its stats.  Its point query takes 4, 2 or 1 lanes per sample from the
+    load: the golden rays repeated R times reach each lane count, and every copy of a ray equals the single run bit for
+    bit.  Every live sample equals the point query at the posed point the march placed it at."""
     import torch
     from instantavatar_b200 import ops
     scene, _ = dev
     inp = train_fwd_golden.inputs(sc, "patch")
-    res = {}
-    try:
-        for k in (1, 2, 4, 0):
-            ops.set_option("query_lanes_per_sample", k)   # lanes sharing a sample's 13 root finds
-            res[k] = train_fwd_golden.run(scene, inp)
-    finally:
-        ops.set_option("query_lanes_per_sample", 0)
-    out0, saved0, st0 = res[1]
+    n = len(inp["o"])
+    out0, saved0, st0 = train_fwd_golden.run(scene, inp)
     assert st0["samples"] > 1000
+    train_fwd_golden.assert_matches("patch", out0, saved0, st0)
     cnt = saved0["count"].long()
     live = torch.arange(saved0["sigma"].shape[1], device="cuda")[None] < cnt[:, None]   # slots the forward filled
-    for k in (2, 4, 0):
-        out1, saved1, st1 = res[k]
-        assert st1["samples"] == st0["samples"] and st1["net_evals"] == st0["net_evals"] and st1["field_loads"] == st0["field_loads"]
+
+    def repeated(R, m):
+        """the first m golden rays repeated R times: every copy of a ray equals the single run; returns the lane count"""
+        rep = {key: (np.concatenate([v[:m]] * R) if isinstance(v, np.ndarray) else v) for key, v in inp.items()}
+        out1, saved1, st1 = train_fwd_golden.run(scene, rep)
+        if m == n:
+            for name in ("samples", "net_evals", "field_loads"):
+                assert st1[name] == R * st0[name], (R, m, name)
+        copies = lambda v: v.view(R, m, *v.shape[1:])
         for name in out0:
-            assert torch.equal(out0[name], out1[name]), (k, name)
-        assert torch.equal(saved0["count"], saved1["count"]) and torch.equal(saved0["best"], saved1["best"])
+            assert all(torch.equal(c, out0[name][:m]) for c in copies(out1[name])), (R, m, name)
+        for name in ("count", "best"):
+            assert all(torch.equal(c, saved0[name][:m]) for c in copies(saved1[name])), (R, m, name)
         for name in ("sigma", "z", "rgb", "xc"):
-            assert torch.equal(saved0[name][live], saved1[name][live]), (k, name)
-    for k, r in res.items():
-        train_fwd_golden.assert_matches("patch", *r)
+            assert all(torch.equal(c[live[:m]], saved0[name][:m][live[:m]]) for c in copies(saved1[name])), (R, m, name)
+        return _list_query_lanes(R * m, st1["samples"])
+
+    covered = {_list_query_lanes(n, st0["samples"])}
+    for want in (2, 1):   # the smallest repeat counts of all rays that take 2 and 1 lanes
+        if want not in covered:
+            R = next(r for r in range(2, 1000) if _list_query_lanes(r * n, r * st0["samples"]) == want)
+            covered.add(repeated(R, n))
+    m = n
+    while 4 not in covered and m > 1:   # a prefix of the rays that takes 4 lanes
+        m //= 2
+        covered.add(repeated(1, m))
+    assert covered == {1, 2, 4}, covered
     # the point query (point mode of the same kernel instantiation) at each live slot's posed point z * d + o, a
     # separate multiply and add as the march computes it
     ray = live.nonzero()[:, 0]

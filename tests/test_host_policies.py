@@ -17,20 +17,19 @@ def test_shard_layout_covers_and_aligns():
             assert L - n < world * 64 + 64                       # padding stays small
 
 
-def test_option_mirror_matches_the_library_and_refuses_retired_options():
+def test_render_option_mirror_matches_the_library_and_refuses_retired_options():
     import ctypes
     import re
     import os
     import pytest
     from instantavatar_b200 import _lib, ops
     src = open(os.path.join(os.path.dirname(ops.__file__), "csrc", "ia_kernels.cu")).read()
-    for name, var in (("render_rays_per_warp", "g_render_rays"), ("query_warps", "g_query_warps"),
-                      ("query_lanes_per_sample", "g_query_lanes")):
-        m = re.search(r"static int %s = (\d+);" % var, src)
-        assert m and int(m.group(1)) == ops._OPTIONS[name], name
-    assert set(ops._OPTIONS) == {"render_rays_per_warp", "query_warps", "query_lanes_per_sample"}
+    m = re.search(r"static int g_render_rays = (\d+);", src)
+    assert m and int(m.group(1)) == ops._OPTIONS["render_rays_per_warp"]
+    assert set(ops._OPTIONS) == {"render_rays_per_warp"}
     # retired options: readable and settable at their one value, never the library's
-    for name, one in (("train_split", 1), ("train_rays_per_warp", 1), ("render_warps", 12)):
+    for name, one in (("train_split", 1), ("train_rays_per_warp", 1), ("render_warps", 12), ("query_warps", 12),
+                      ("query_lanes_per_sample", 0)):
         assert ops.get_option(name) == one
         ops.set_option(name, one)
         for value in (0, 1, 2, 4, 8, 16, 20):
@@ -40,12 +39,11 @@ def test_option_mirror_matches_the_library_and_refuses_retired_options():
         assert ops.get_option(name) == one
     # ... and unknown to the library, even at the value it used to default to
     for name, value in ((b"train_rays_per_warp", 1), (b"render_plan", 1), (b"occupancy_lanes_per_point", 0),
-                        (b"render_warps", 12)):
+                        (b"render_warps", 12), (b"query_warps", 12), (b"query_lanes_per_sample", 0)):
         assert _lib.lib().ia_set_option(name, ctypes.c_int(value)) == -1, name
         assert b"unknown option" in _lib.lib().ia_last_error(), name
     # retired values of the remaining options are refused
-    for name, value in ((b"render_rays_per_warp", 8), (b"render_rays_per_warp", 16), (b"render_rays_per_warp", 32),
-                        (b"query_warps", 20)):
+    for name, value in ((b"render_rays_per_warp", 8), (b"render_rays_per_warp", 16), (b"render_rays_per_warp", 32)):
         assert _lib.lib().ia_set_option(name, ctypes.c_int(value)) == -1, (name, value)
         assert b"invalid argument" in _lib.lib().ia_last_error(), (name, value)
     # every option bench.py reports is readable
