@@ -612,6 +612,26 @@ int ia_shade_composite(const float* verts, int F, int n_verts, const int* faces,
                        const int* face_id, const float* bary, void* workspace, size_t workspace_bytes, uint8_t* frames,
                        ia_stream_t stream);
 
+/* Mask clean-up of a custom sequence: the per-frame body of scripts/custom/extract-largest-connected-components.py
+ * (cv2.threshold(img, 0, 255, THRESH_BINARY), morphologyEx MORPH_OPEN then MORPH_CLOSE with a 5x5 all-ones kernel,
+ * connectedComponentsWithStats(connectivity=8), the arg-max area and img[~mask] = 0) for F frames of one size H x W
+ * (DESIGN.md §3.5, §5.12).
+ *
+ * masks [F][H][W] uint8: the grayscale values; v > 0 is foreground.  Erosion reads pixels outside the image as
+ * foreground, dilation as background (cv2's default border).  mask_out [F][H][W] uint8 receives 255 on the kept
+ * component and 0 elsewhere.  images / images_out [F][H][W][3] uint8 are both NULL or both set; images_out may alias
+ * images and receives the image with every pixel outside the kept component zeroed.  stats [F][2] int32 receives the
+ * number of 8-connected components after the closing (cv2's num_labels - 1) and the kept component's area.  The largest
+ * area is kept; an exact tie goes to the component whose first pixel in raster order (lowest y*W + x) is lowest.  A
+ * frame with no foreground after the closing gets an all-zero mask and image and a kept area of 0.
+ * workspace: device, 256-byte aligned, ia_mask_workspace_bytes(F, H, W) bytes (0 for F = 0 and invalid sizes), about
+ * 12 bytes a pixel.  No host synchronisation; two calls on the same input give identical results.
+ * IA_EINVAL: H or W < 1, F < 0, F*H*W >= 2^31, a short workspace, a NULL pointer, one of images / images_out NULL.  F = 0
+ * does nothing. */
+size_t ia_mask_workspace_bytes(int F, int H, int W);
+int ia_mask_largest_component(const uint8_t* masks, int F, int H, int W, uint8_t* mask_out, const uint8_t* images,
+                              uint8_t* images_out, int* stats, void* workspace, size_t workspace_bytes, ia_stream_t stream);
+
 #ifdef __cplusplus
 }
 #endif

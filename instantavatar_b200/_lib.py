@@ -33,6 +33,7 @@ SYMBOLS = [
     "ia_test_panel", "ia_image_metrics", "ia_gif_quantize_workspace_bytes", "ia_gif_quantize",
     "ia_smpl_fit_workspace_bytes", "ia_smpl_fit_forward", "ia_smpl_fit_objective",
     "ia_raster_workspace_bytes", "ia_raster", "ia_shade_composite",
+    "ia_mask_workspace_bytes", "ia_mask_largest_component",
 ]
 
 
@@ -96,6 +97,7 @@ def lib():
         _lib.ia_gif_quantize_workspace_bytes.restype = C.c_size_t
         _lib.ia_smpl_fit_workspace_bytes.restype = C.c_size_t
         _lib.ia_raster_workspace_bytes.restype = C.c_size_t
+        _lib.ia_mask_workspace_bytes.restype = C.c_size_t
         for s in SYMBOLS:
             getattr(_lib, s)  # fail loudly on a stale library
         if _lib.ia_abi_version() != 1:

@@ -982,6 +982,50 @@ def shade_composite(frames, verts, faces, csr, raster: dict, K, E, workspace=Non
     return frames
 
 
+# pixels per ia_mask_largest_component call: below its 2^31 index limit, and a workspace of about 3 GB (12 B a pixel)
+MASK_PIXELS_PER_CALL = 1 << 28
+
+
+def mask_largest_component(masks, images=None, images_out=None):
+    """extract-largest-connected-components.py's per-frame body (include/ia_b200.h, ia_mask_largest_component; DESIGN.md
+    §3.5): masks [F,H,W] uint8 (device; v > 0 is foreground) -> (mask_out [F,H,W] uint8 0/255, images_out, stats [F,2]
+    int32 = (components after the closing, kept area)).  The largest 8-connected component of the opened-then-closed mask
+    is kept, exact ties to the lowest first pixel in raster order; a frame left empty keeps nothing (area 0).
+    images [F,H,W,3] uint8 (optional) -> images_out (a new tensor, or the given one, which may be `images` itself) with
+    the pixels outside the kept component zeroed; None without images.  Frames go through in calls of at most
+    MASK_PIXELS_PER_CALL pixels; no host synchronisation."""
+    if masks.dtype != torch.uint8 or masks.dim() != 3:
+        raise ValueError(f"mask_largest_component: masks must be uint8 [F,H,W], got {masks.dtype} {tuple(masks.shape)}")
+    F, H, W = masks.shape
+    if H < 1 or W < 1:
+        raise ValueError(f"mask_largest_component: frames must be at least 1x1, got {H}x{W}")
+    if H * W >= 2 ** 31:
+        raise ValueError(f"mask_largest_component: one {H}x{W} frame exceeds the kernels' 2^31 index limit")
+    if images is not None and (images.dtype != torch.uint8 or tuple(images.shape) != (F, H, W, 3)):
+        raise ValueError(f"mask_largest_component: images must be uint8 {(F, H, W, 3)}, got {images.dtype} "
+                         f"{tuple(images.shape)}")
+    if images_out is not None and (images is None or images_out.dtype != torch.uint8 or images_out.shape != images.shape):
+        raise ValueError("mask_largest_component: images_out needs images and must match their dtype and shape")
+    dev = masks.device
+    mask_out = torch.empty_like(masks)
+    stats = torch.empty((F, 2), device=dev, dtype=torch.int32)
+    if images is not None and images_out is None:
+        images_out = torch.empty_like(images)
+    chunk = max(1, MASK_PIXELS_PER_CALL // (H * W))
+    workspace = None
+    for s in range(0, F, chunk):
+        n = min(chunk, F - s)
+        nbytes = int(lib().ia_mask_workspace_bytes(C.c_int(n), C.c_int(H), C.c_int(W)))
+        if workspace is None or workspace.numel() < nbytes:
+            workspace = torch.empty(nbytes, device=dev, dtype=torch.uint8)
+        sl = lambda t: None if t is None else t[s:s + n]
+        _lib.count(9); check(lib().ia_mask_largest_component(ptr(sl(masks)), C.c_int(n), C.c_int(H), C.c_int(W),
+                                                             ptr(sl(mask_out)), ptr(sl(images)), ptr(sl(images_out)),
+                                                             ptr(sl(stats), torch.int32), ptr(workspace),
+                                                             C.c_size_t(workspace.numel()), stream()))
+    return mask_out, images_out, stats
+
+
 # ------------------------------------------------------------------------------------------------------------------
 # device guard: every operator launches on the current stream OF THE DEVICE ITS TENSORS LIVE ON (one process may hold
 # tensors on several GPUs; function attributes and SM counts are cached per device inside the library)
