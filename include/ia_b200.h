@@ -369,6 +369,16 @@ int ia_skin_points(const float* lbs_voxel, int D, int H, int W, const float* off
                    const float* tfs, int n_frames, const float* xc, int n, float* xd, float* weights /*nullable*/,
                    ia_stream_t stream);
 
+/* Per-vertex skinning weights for a rig (DESIGN.md §3, "Rigged export").  Each vertex of xc [n][3] samples its 24 weights
+ * exactly as ia_skin_points does, keeps the K largest in descending order (a tie goes to the lower joint index) and
+ * divides them by their sum, accumulated in stored order: joints [n][K] uint8, weights [n][K].  A kept weight of exactly 0
+ * is stored as joint 0, weight 0.  dropped [n] (nullable) receives the sum of the 24 - K weights not kept, in joint order.
+ * A vertex whose kept sum is not positive gets joint 0 with weight 1 (then zeros) and adds 1 to *n_fallback (device int,
+ * accumulated).  n = 0: nothing is done; K not in {4, 8, ..., 24}, n < 0 or D / H / W < 1: IA_EINVAL. */
+int ia_vertex_skin_weights(const float* lbs_voxel, int D, int H, int W, const float* offset_k, const float* scale_k,
+                           const float* xc, int n, int K, uint8_t* joints, float* weights, float* dropped /*nullable*/,
+                           int* n_fallback, ia_stream_t stream);
+
 /* Pose gradient of the nearest-vertex deformer (scene->nv set).  For each of the first min(*count, capacity) list samples
  * of ia_composite_bwd with best >= 0: l_rz [capacity][3] holds (ray index, z, 0) -- what ia_composite_bwd writes into l_xd
  * when it is given the rays rays_o[i] = (i, 0, 0), rays_d[i] = (0, 1, 0) (z * 0 + i and z * 1 + 0 are exact).  The posed
@@ -611,6 +621,11 @@ int ia_shade_composite(const float* verts, int F, int n_verts, const int* faces,
                        const int* csr_faces, const float* K /*[host]*/, const float* E /*[host]*/, int H, int W,
                        const int* face_id, const float* bary, void* workspace, size_t workspace_bytes, uint8_t* frames,
                        ia_stream_t stream);
+/* ia_vertex_normals: normals [V][3] of one mesh verts [V][3], computed by ia_shade_composite's normal pass (area-weighted
+ * face normals summed in csr order, normalised; 0 where they cancel), so bit-identical to the normals it shades with.
+ * V = 0: nothing is done; a negative V or NF, a NULL pointer: IA_EINVAL. */
+int ia_vertex_normals(const float* verts, int n_verts, const int* faces, int n_faces, const int* csr_offsets,
+                      const int* csr_faces, float* normals, ia_stream_t stream);
 
 /* Mask clean-up of a custom sequence: the per-frame body of scripts/custom/extract-largest-connected-components.py
  * (cv2.threshold(img, 0, 255, THRESH_BINARY), morphologyEx MORPH_OPEN then MORPH_CLOSE with a 5x5 all-ones kernel,

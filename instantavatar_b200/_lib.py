@@ -34,6 +34,7 @@ SYMBOLS = [
     "ia_smpl_fit_workspace_bytes", "ia_smpl_fit_forward", "ia_smpl_fit_objective",
     "ia_raster_workspace_bytes", "ia_raster", "ia_shade_composite",
     "ia_mask_workspace_bytes", "ia_mask_largest_component",
+    "ia_vertex_skin_weights", "ia_vertex_normals",
 ]
 
 

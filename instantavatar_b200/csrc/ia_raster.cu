@@ -9,7 +9,7 @@
 //                        a ballot compacts the hits (order kept) into shared memory, then every pixel tests them in
 //                        order with a strict < on depth.  No lists, no atomics, no host reads: the lowest index wins a
 //                        tie and two runs are bit-identical.
-// ia_shade_composite, two launches:
+// ia_shade_composite, two launches (ia_vertex_normals runs the first alone, on one mesh):
 //   vertex_normal_kernel: per (frame, vertex) the area-weighted face normals summed over the vertex's faces in the
 //                         order of the caller's vertex -> face CSR, normalised.
 //   shade_kernel:         per pixel with a face: the perspective-correct normal, two-sided Lambert with a headlight,
@@ -324,6 +324,18 @@ extern "C" int ia_shade_composite(const float* verts, int F, int n_verts, const 
     const long hw = (long)H * W;
     shade_kernel<<<dim3((unsigned)((hw + kShadeThreads - 1) / kShadeThreads), F), kShadeThreads, 0, st>>>(
         faces, n_verts, normals, face_id, reinterpret_cast<const float2*>(bary), H, W, cam, frames);
+    IA_CHECK_CUDA(cudaPeekAtLastError());
+    return IA_OK;
+}
+
+extern "C" int ia_vertex_normals(const float* verts, int n_verts, const int* faces, int n_faces, const int* csr_offsets,
+                                 const int* csr_faces, float* normals, ia_stream_t stream) {
+    IA_REQUIRE(valid_sizes(1, n_verts, n_faces));
+    if (n_verts == 0) return IA_OK;
+    IA_REQUIRE(verts && csr_offsets && normals && (n_faces == 0 || (faces && csr_faces)));
+    // the shading pass's own kernel, one frame: the normals are bit-identical to those ia_shade_composite shades with
+    vertex_normal_kernel<<<dim3((n_verts + kShadeThreads - 1) / kShadeThreads, 1), kShadeThreads, 0, (cudaStream_t)stream>>>(
+        verts, faces, n_verts, csr_offsets, csr_faces, normals);
     IA_CHECK_CUDA(cudaPeekAtLastError());
     return IA_OK;
 }

@@ -1306,7 +1306,72 @@ __global__ void __launch_bounds__(256) skin_points_kernel(const __grid_constant_
         }
     }
 }
+
+struct VertexWeightArgs {
+    const float* lbs_voxel; int D, H, W;
+    const float* offset_k; const float* scale_k;
+    const float* xc; int n, K;
+    uint8_t* joints; float* weights; float* dropped; int* n_fallback;
+};
+
+// The K strongest of a vertex's 24 sampled skinning weights (DESIGN.md §3 "Rigged export"): K passes, each taking the
+// largest weight not yet taken (strict >, so the lower joint index wins a tie), stored in descending order; then divided
+// by their sum, accumulated in stored order.  A zero weight is stored as joint 0, weight 0.  A vertex whose kept sum is
+// not positive falls back to joint 0 with weight 1 and is counted.
+__global__ void __launch_bounds__(256) vertex_skin_weights_kernel(const __grid_constant__ VertexWeightArgs a) {
+    const int p = blockIdx.x * blockDim.x + threadIdx.x;
+    if (p >= a.n) return;
+    const float x[3] = {a.xc[(long)p * 3], a.xc[(long)p * 3 + 1], a.xc[(long)p * 3 + 2]};
+    const float q[3] = {a.scale_k[0] * (x[0] + a.offset_k[0]), a.scale_k[1] * (x[1] + a.offset_k[1]), a.scale_k[2] * (x[2] + a.offset_k[2])};
+    float wts[24];
+#pragma unroll
+    for (int j = 0; j < 24; j++) wts[j] = 0.f;
+    sample_lbs_weights(a.lbs_voxel, a.D, a.H, a.W, (long)a.D * a.H * a.W, q, wts);
+    uint8_t* jo = a.joints + (long)p * a.K;
+    float* wo = a.weights + (long)p * a.K;
+    unsigned taken = 0u;
+    float sum = 0.f;
+    for (int k = 0; k < a.K; k++) {
+        int best = -1;
+        float bw = 0.f;
+#pragma unroll
+        for (int j = 0; j < 24; j++)
+            if (!((taken >> j) & 1u) && (best < 0 || wts[j] > bw)) { best = j; bw = wts[j]; }
+        taken |= 1u << best;
+        const float w = bw == 0.f ? 0.f : bw;
+        jo[k] = w == 0.f ? 0 : (uint8_t)best;
+        wo[k] = w;
+        sum += w;
+    }
+    if (a.dropped) {
+        float d = 0.f;
+#pragma unroll
+        for (int j = 0; j < 24; j++) d += ((taken >> j) & 1u) ? 0.f : wts[j];
+        a.dropped[p] = d;
+    }
+    if (!(sum > 0.f)) {
+        for (int k = 0; k < a.K; k++) { jo[k] = 0; wo[k] = k == 0 ? 1.f : 0.f; }
+        atomicAdd(a.n_fallback, 1);
+        return;
+    }
+    for (int k = 0; k < a.K; k++) wo[k] = wo[k] / sum;
+}
 }  // namespace
+
+extern "C" int ia_vertex_skin_weights(const float* lbs_voxel, int D, int H, int W, const float* offset_k, const float* scale_k,
+                                      const float* xc, int n, int K, uint8_t* joints, float* weights, float* dropped,
+                                      int* n_fallback, ia_stream_t stream) {
+    IA_REQUIRE(D > 0 && H > 0 && W > 0 && n >= 0);
+    IA_REQUIRE(K >= 4 && K <= 24 && K % 4 == 0);
+    if (n == 0) return IA_OK;
+    IA_REQUIRE(lbs_voxel && offset_k && scale_k && xc && joints && weights && n_fallback);
+    VertexWeightArgs a;
+    a.lbs_voxel = lbs_voxel; a.D = D; a.H = H; a.W = W; a.offset_k = offset_k; a.scale_k = scale_k;
+    a.xc = xc; a.n = n; a.K = K; a.joints = joints; a.weights = weights; a.dropped = dropped; a.n_fallback = n_fallback;
+    vertex_skin_weights_kernel<<<(unsigned)((n + 255) / 256), 256, 0, (cudaStream_t)stream>>>(a);
+    IA_CHECK_CUDA(cudaPeekAtLastError());
+    return IA_OK;
+}
 
 extern "C" int ia_skin_points(const float* lbs_voxel, int D, int H, int W, const float* offset_k, const float* scale_k,
                               const float* tfs, int n_frames, const float* xc, int n, float* xd, float* weights,

@@ -177,14 +177,19 @@ class SNARFDeformer:
         self.fast_prepare = True  # per-frame bone transforms through ia_smpl_tfs (False: full SMPL forward in torch)
         self._vertices = None
 
-    def initialize(self, betas, device, lbs_voxel=None):
-        """snarf_deformer.py:41-69"""
+    def canonical_body_pose(self, device):
+        """body_pose [1,69] of the canonical pose the skinning field lives in: opt.cano_pose by name, or its four numbers
+        (hip and shoulder z-rotations) (snarf_deformer.py:42-48)"""
         cano = _opt_get(self.opt, "cano_pose", "A_pose")
         if isinstance(cano, str):
-            body_pose_t = get_predefined_rest_pose(cano, device=device)
-        else:
-            body_pose_t = torch.zeros((1, 69), device=device)
-            body_pose_t[:, 2] = cano[0]; body_pose_t[:, 5] = cano[1]; body_pose_t[:, 47] = cano[2]; body_pose_t[:, 50] = cano[3]
+            return get_predefined_rest_pose(cano, device=device)
+        body_pose_t = torch.zeros((1, 69), device=device)
+        body_pose_t[:, 2] = cano[0]; body_pose_t[:, 5] = cano[1]; body_pose_t[:, 47] = cano[2]; body_pose_t[:, 50] = cano[3]
+        return body_pose_t
+
+    def initialize(self, betas, device, lbs_voxel=None):
+        """snarf_deformer.py:41-69"""
+        body_pose_t = self.canonical_body_pose(device)
         out = self.body_model(betas=betas[:1], body_pose=body_pose_t)
         self.tfs_inv_t = torch.inverse(out.A.float().detach())
         self.vs_template = out.vertices

@@ -222,14 +222,20 @@ def avatar_mesh(deformer, net, resolution=256, *, level_set, space="canonical", 
     return to_mesh(verts, faces, rgb)
 
 
-def pose_tfs(deformer, poses) -> torch.Tensor:
-    """bone transforms [F,24,4,4] of F poses (SMPL dicts with a leading F dimension: global_orient [F,3], body_pose
-    [F,69], transl [F,3] or absent) from ia_smpl_tfs, the kernel SNARFDeformer.prepare_deformer renders with"""
+def require_skinning_field(deformer):
+    """refuse a deformer without a voxelised skinning field: TypeError for anything but a SNARFDeformer, RuntimeError
+    before its prepare_deformer has run"""
     from .deformers.snarf_deformer import SNARFDeformer
     if not isinstance(deformer, SNARFDeformer):
         raise TypeError(f"skinning needs the voxelised skinning weights of a SNARFDeformer, got {type(deformer).__name__}")
     if not deformer.initialized:
         raise RuntimeError("prepare_deformer has not run: the subject's skinning field does not exist yet")
+
+
+def pose_tfs(deformer, poses) -> torch.Tensor:
+    """bone transforms [F,24,4,4] of F poses (SMPL dicts with a leading F dimension: global_orient [F,3], body_pose
+    [F,69], transl [F,3] or absent) from ia_smpl_tfs, the kernel SNARFDeformer.prepare_deformer renders with"""
+    require_skinning_field(deformer)
     dev = deformer.joints_rest.device
     body_pose = torch.as_tensor(poses["body_pose"], dtype=torch.float32, device=dev).reshape(-1, 69)
     n = body_pose.shape[0]
@@ -258,3 +264,6 @@ def skin_mesh(m: Mesh, deformer, poses) -> list:
         posed.faces, posed.vertex_colors = m.faces, m.vertex_colors
         out.append(posed)
     return out
+
+
+from .rig import export_glb, rig_weights, skeleton  # noqa: E402,F401  (rigged glTF export, rig.py)

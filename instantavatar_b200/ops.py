@@ -592,6 +592,29 @@ def skin_points(lbs_voxel, offset_k, scale_k, tfs, xc, want_weights=False):
     return (xd, weights) if want_weights else xd
 
 
+RIG_INFLUENCES = (4, 8, 12, 16, 20, 24)
+
+
+def vertex_skin_weights(lbs_voxel, offset_k, scale_k, xc, K: int = 4, want_dropped=False):
+    """the K strongest skinning weights of each canonical point xc [n,3] (ia_vertex_skin_weights; DESIGN.md §3 "Rigged
+    export"): sampled as skin_points samples them, kept in descending order (ties to the lower joint), renormalised by
+    their sum -> (joints uint8 [n,K], weights [n,K], n_fallback int32 [1] (device), dropped [n] with want_dropped)"""
+    if K not in RIG_INFLUENCES:
+        raise ValueError(f"influences must be one of {RIG_INFLUENCES}, got {K!r}")
+    D, H, W = lbs_voxel.shape[-3:]
+    xc = xc.reshape(-1, 3).contiguous()
+    n, dev = xc.shape[0], xc.device
+    joints = torch.empty((n, K), device=dev, dtype=torch.uint8)
+    weights = torch.empty((n, K), device=dev, dtype=f32)
+    dropped = torch.empty(n, device=dev, dtype=f32) if want_dropped else None
+    n_fallback = torch.zeros(1, device=dev, dtype=torch.int32)
+    _lib.count(1); check(lib().ia_vertex_skin_weights(ptr(lbs_voxel.reshape(24, D, H, W).contiguous(), f32), C.c_int(D), C.c_int(H),
+                                                      C.c_int(W), ptr(offset_k.reshape(3).contiguous(), f32),
+                                                      ptr(scale_k.reshape(3).contiguous(), f32), ptr(xc, f32), C.c_int(n), C.c_int(K),
+                                                      ptr(joints), ptr(weights), ptr(dropped), ptr(n_fallback, torch.int32), stream()))
+    return (joints, weights, n_fallback, dropped) if want_dropped else (joints, weights, n_fallback)
+
+
 _RAY_SLOT_CODES: dict = {}
 
 
@@ -980,6 +1003,17 @@ def shade_composite(frames, verts, faces, csr, raster: dict, K, E, workspace=Non
                                                   C.c_int(W), ptr(raster["face_id"], torch.int32), ptr(raster["bary"], f32),
                                                   ptr(workspace), C.c_size_t(workspace.numel()), ptr(frames), stream()))
     return frames
+
+
+def vertex_normals(verts, faces, csr):
+    """area-weighted vertex normals [V,3] of one mesh verts [V,3] fp32, faces [NF,3] int32 (device), csr = face_csr(faces)
+    (ia_vertex_normals): the normal pass of shade_composite, bit for bit.  One launch."""
+    V, NF = verts.shape[0], faces.shape[0]
+    normals = torch.empty((V, 3), device=verts.device, dtype=f32)
+    _lib.count(1); check(lib().ia_vertex_normals(ptr(verts.contiguous(), f32), C.c_int(V), ptr(faces.contiguous(), torch.int32),
+                                                 C.c_int(NF), ptr(csr[0], torch.int32), ptr(csr[1], torch.int32), ptr(normals),
+                                                 stream()))
+    return normals
 
 
 # pixels per ia_mask_largest_component call: below its 2^31 index limit, and a workspace of about 3 GB (12 B a pixel)
