@@ -9,7 +9,7 @@ import numpy as np
 import torch
 
 from . import _lib
-from ._lib import IaNearestVertex, IaScene, IaStats, check, lib, ptr, stream
+from ._lib import STREAM, IaNearestVertex, IaScene, call, ptr
 
 f32 = torch.float32
 
@@ -31,9 +31,8 @@ def precompute(voxel_w: torch.Tensor, tfs: torch.Tensor, offset_k: torch.Tensor,
     buf = torch.empty(D * H * (W + 1) * 12, device=dev, dtype=f32)
     vd = torch.empty((3, D, H, W), device=dev, dtype=f32) if want_voxel_d else None
     aabb = torch.empty(6, device=dev, dtype=f32)  # initialised by the library
-    _lib.count(1); check(lib().ia_precompute(ptr(voxel_w, f32), ptr(tfs.reshape(24, 4, 4).contiguous(), f32),
-                              ptr(offset_k.reshape(3).contiguous(), f32), ptr(scale_k.reshape(3).contiguous(), f32),
-                              C.c_int(D), C.c_int(H), C.c_int(W), ptr(buf), ptr(vd), ptr(aabb), stream()))
+    _lib.count(1); call("ia_precompute", voxel_w, tfs.reshape(24, 4, 4).contiguous(), offset_k.reshape(3).contiguous(),
+                        scale_k.reshape(3).contiguous(), D, H, W, buf, vd, aabb, STREAM)
     return buf.as_strided((D, H, W, 24), _field_strides(H, W)), vd, aabb
 
 
@@ -57,16 +56,15 @@ def params_to_half(enc_params: torch.Tensor, col_params: torch.Tensor, table_h=N
         table_h = torch.empty((total, 2), device=dev, dtype=torch.float16)
     if mlp_h is None:
         mlp_h = torch.empty(_lib.IA_MLP_HALFS, device=dev, dtype=torch.float16)
-    _lib.count(1); check(lib().ia_params_to_half(ptr(enc_params, f32), ptr(col_params, f32), ptr(table_h), ptr(mlp_h), stream()))
+    _lib.count(1); call("ia_params_to_half", enc_params, col_params, table_h, mlp_h, STREAM)
     return table_h, mlp_h
 
 
 def pack_occupancy(field_bool: torch.Tensor, bits=None):
     G = field_bool.shape[0]
-    fb = field_bool.contiguous().view(torch.uint8) if field_bool.dtype == torch.bool else field_bool.contiguous()
     if bits is None:
-        bits = torch.empty(G * G * G // 32 + 8, device=fb.device, dtype=torch.int32)
-    _lib.count(2); check(lib().ia_pack_occupancy(ptr(fb), ptr(bits), C.c_int(G), stream()))
+        bits = torch.empty(G * G * G // 32 + 8, device=field_bool.device, dtype=torch.int32)
+    _lib.count(2); call("ia_pack_occupancy", field_bool.contiguous(), bits, G, STREAM)
     return bits
 
 
@@ -82,23 +80,21 @@ def occupancy_build(density: torch.Tensor, bits=None, want_field=True, workspace
     nbytes = 12 * G * G * G + 64
     if workspace is None or workspace.numel() < nbytes:
         workspace = torch.empty(nbytes, device=dev, dtype=torch.uint8)
-    _lib.count(7); check(lib().ia_occupancy_build(ptr(density, f32), C.c_int(G), ptr(field), ptr(bits), ptr(workspace), C.c_size_t(nbytes), stream()))
+    _lib.count(7); call("ia_occupancy_build", density, G, field, bits, workspace, nbytes, STREAM)
     return field, bits
 
 
 def mc_count(field: torch.Tensor, level: float, workspace=None):
     """marching cubes, first call: field [nx,ny,nz] fp32 -> (counts int64 [3] = n_verts, n_faces, n_nonfinite (device),
     workspace holding the classification and scans for mc_emit)"""
-    fp = ptr(field, f32)
     nx, ny, nz = field.shape
-    nbytes = lib().ia_mc_workspace_bytes(nx, ny, nz)
+    nbytes = call("ia_mc_workspace_bytes", nx, ny, nz)
     if nbytes == 0:
         raise RuntimeError(f"libia_b200: marching cubes needs a lattice of at least 2x2x2 with 3*nx*ny*nz < 2^31, got {tuple(field.shape)}")
     if workspace is None or workspace.numel() < nbytes:
         workspace = torch.empty(nbytes, device=field.device, dtype=torch.uint8)
     counts = torch.empty(3, device=field.device, dtype=torch.int64)
-    _lib.count(6); check(lib().ia_mc_count(fp, nx, ny, nz, C.c_float(level), ptr(workspace), C.c_size_t(nbytes),
-                                           ptr(counts, torch.int64), stream()))
+    _lib.count(6); call("ia_mc_count", field, nx, ny, nz, level, workspace, nbytes, counts, STREAM)
     return counts, workspace
 
 
@@ -110,9 +106,8 @@ def mc_emit(field: torch.Tensor, level: float, workspace, n_verts: int, n_faces:
     dev = field.device
     verts = torch.empty((n_verts, 3), device=dev, dtype=f32)
     faces = torch.empty((n_faces, 3), device=dev, dtype=torch.int32)
-    _lib.count(2); check(lib().ia_mc_emit(ptr(field, f32), nx, ny, nz, C.c_float(level), C.c_int(1 if flip else 0), C.c_float(div),
-                                          ptr(ext_origin, f32), ptr(workspace), C.c_size_t(workspace.numel()), C.c_int(n_verts),
-                                          C.c_int(n_faces), ptr(verts), ptr(faces), stream()))
+    _lib.count(2); call("ia_mc_emit", field, nx, ny, nz, level, 1 if flip else 0, div, ext_origin, workspace, workspace.numel(),
+                        n_verts, n_faces, verts, faces, STREAM)
     return verts, faces
 
 
@@ -121,14 +116,13 @@ def mc_largest_component(verts: torch.Tensor, faces: torch.Tensor):
     Reads the kept counts back (one device synchronisation)."""
     V, F = verts.shape[0], faces.shape[0]
     dev = verts.device
-    nbytes = lib().ia_mc_component_workspace_bytes(V, F)
+    nbytes = call("ia_mc_component_workspace_bytes", V, F)
     if nbytes == 0:
         raise RuntimeError(f"libia_b200: component extraction needs 0 < V, F < 2^31 - 1, got V={V}, F={F}")
     workspace = torch.empty(nbytes, device=dev, dtype=torch.uint8)
     verts_out = torch.empty_like(verts); faces_out = torch.empty_like(faces)
     kept = torch.empty(2, device=dev, dtype=torch.int64)
-    _lib.count(12); check(lib().ia_mc_largest_component(ptr(verts, f32), ptr(faces, torch.int32), C.c_int(V), C.c_int(F), ptr(workspace),
-                                                       C.c_size_t(nbytes), ptr(verts_out), ptr(faces_out), ptr(kept), stream()))
+    _lib.count(12); call("ia_mc_largest_component", verts, faces, V, F, workspace, nbytes, verts_out, faces_out, kept, STREAM)
     kv, kf = kept.tolist()
     return verts_out[:kv], faces_out[:kf]
 
@@ -136,7 +130,7 @@ def mc_largest_component(verts: torch.Tensor, faces: torch.Tensor):
 def occupancy_query_workspace_bytes(G: int, passes: int, n_shards: int = 1) -> int:
     """bytes of the occupancy pass's workspace: counters and the root list, which holds the worst case of the shard
     (every one of a grid point's 13 root finds kept)"""
-    return int(lib().ia_occupancy_query_workspace_bytes(C.c_int(G), C.c_int(passes), C.c_int(n_shards)))
+    return call("ia_occupancy_query_workspace_bytes", G, passes, n_shards)
 
 
 def occupancy_query(scene, jitters: torch.Tensor, aabb6: torch.Tensor, density=None, stats=None, workspace=None, shard=(0, 1), peer=None):
@@ -153,14 +147,13 @@ def occupancy_query(scene, jitters: torch.Tensor, aabb6: torch.Tensor, density=N
         raise ValueError(f"occupancy_query: workspace of {workspace.numel() * workspace.element_size()} bytes, needs {nbytes}")
     s = scene.c_struct()
     if peer is not None:
-        _lib.count(1); check(lib().ia_occupancy_query_peer(C.byref(s), ptr(jitters.contiguous(), f32), ptr(aabb6, f32), C.c_int(G), C.c_int(P),
-                                                           C.c_void_p(int(peer[0])), C.c_int(int(peer[1])), ptr(workspace), C.c_int(shard[0]),
-                                                           C.c_int(shard[1]), ptr(stats), stream()))
+        _lib.count(1); call("ia_occupancy_query_peer", C.byref(s), jitters.contiguous(), aabb6, G, P, int(peer[0]), int(peer[1]),
+                            workspace, shard[0], shard[1], stats, STREAM)
         return None
     if density is None:
         density = torch.empty((G, G, G), device=jitters.device, dtype=f32)
-    _lib.count(1); check(lib().ia_occupancy_query(C.byref(s), ptr(jitters.contiguous(), f32), ptr(aabb6, f32), C.c_int(G), C.c_int(P),
-                                                  ptr(density), ptr(workspace), C.c_int(shard[0]), C.c_int(shard[1]), ptr(stats), stream()))
+    _lib.count(1); call("ia_occupancy_query", C.byref(s), jitters.contiguous(), aabb6, G, P, density, workspace, shard[0], shard[1],
+                        stats, STREAM)
     return density
 
 
@@ -181,7 +174,7 @@ class NearestVertex:
 
 
 def nv_workspace_bytes(n_verts: int) -> int:
-    return int(lib().ia_nv_workspace_bytes(C.c_int(n_verts)))
+    return call("ia_nv_workspace_bytes", n_verts)
 
 
 def nv_grid_build(nv: NearestVertex) -> NearestVertex:
@@ -190,7 +183,7 @@ def nv_grid_build(nv: NearestVertex) -> NearestVertex:
     if nv.grid is None or nv.grid.numel() < nbytes:
         nv.grid = torch.empty(nbytes, device=nv.verts.device, dtype=torch.uint8)
     s = nv.c_struct()
-    _lib.count(1); check(lib().ia_nv_grid_build(C.byref(s), stream()))
+    _lib.count(1); call("ia_nv_grid_build", C.byref(s), STREAM)
     return nv
 
 
@@ -200,7 +193,7 @@ def nv_nearest(nv: NearestVertex, pts):
     n = pts.shape[0]
     idx = torch.empty(n, device=pts.device, dtype=torch.int32); d2 = torch.empty(n, device=pts.device, dtype=f32)
     s = nv.c_struct()
-    _lib.count(1); check(lib().ia_nv_nearest(C.byref(s), ptr(pts, f32), C.c_int(n), ptr(idx, torch.int32), ptr(d2), stream()))
+    _lib.count(1); call("ia_nv_nearest", C.byref(s), pts, n, idx, d2, STREAM)
     return d2, idx.long()
 
 
@@ -251,8 +244,7 @@ def gather_ceiling(field: torch.Tensor, iters: int = 200, warps: int = 12, coher
         cnt.zero_()
         e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
         e0.record()
-        _lib.count(1); check(lib().ia_gather_ceiling(fp, C.c_int(D), C.c_int(H), C.c_int(W), C.c_int(iters), C.c_int(warps),
-                                                     C.c_int(1 if coherent else 0), ptr(cnt), None, stream()))
+        _lib.count(1); call("ia_gather_ceiling", fp, D, H, W, iters, warps, 1 if coherent else 0, cnt, None, STREAM)
         e1.record()
         e1.synchronize()
         ms = e0.elapsed_time(e1)
@@ -278,7 +270,7 @@ def set_option(name: str, value: int):
         if int(value) != _FIXED_OPTIONS[name]:
             raise ValueError(f"{name} can only be {_FIXED_OPTIONS[name]}: the other kernels it selected were retired")
         return
-    check(lib().ia_set_option(name.encode(), C.c_int(value)))
+    call("ia_set_option", name.encode(), value)
     _OPTIONS[name] = int(value)
 
 
@@ -306,19 +298,14 @@ def render_fwd(scene: Scene, rays_o, rays_d, near, far, bg=None, image_width: in
         out = {"rgb": torch.empty((n, 3), device=dev, dtype=f32), "depth": torch.empty(n, device=dev, dtype=f32),
                "alpha": torch.empty(n, device=dev, dtype=f32), "counter": torch.empty(n, device=dev, dtype=f32)}
     if workspace is None:
-        workspace = torch.empty(int(lib().ia_render_workspace_bytes(C.c_int(n))), device=dev, dtype=torch.uint8)
+        workspace = torch.empty(call("ia_render_workspace_bytes", n), device=dev, dtype=torch.uint8)
     s = scene.c_struct()
+    args = (C.byref(s), rays_o, rays_d, near, far, n, bg, image_width, out["rgb"], out["depth"], out["alpha"], out["counter"],
+            workspace, workspace.numel() * workspace.element_size(), stats)
     if peer is not None:
-        _lib.count(3); check(lib().ia_render_fwd_peer(C.byref(s), ptr(rays_o, f32), ptr(rays_d, f32), ptr(near, f32), ptr(far, f32), C.c_int(n),
-                                  ptr(bg), C.c_int(image_width), ptr(out["rgb"]), ptr(out["depth"]), ptr(out["alpha"]),
-                                  ptr(out["counter"]), ptr(workspace), C.c_size_t(workspace.numel() * workspace.element_size()),
-                                  ptr(stats), ptr(peer[0], torch.int32) if peer[0] is not None else None, C.c_void_p(int(peer[1])),
-                                  C.c_int(int(peer[2])), stream()))
+        _lib.count(3); call("ia_render_fwd_peer", *args, peer[0], int(peer[1]), int(peer[2]), STREAM)
         return out
-    _lib.count(3); check(lib().ia_render_fwd(C.byref(s), ptr(rays_o, f32), ptr(rays_d, f32), ptr(near, f32), ptr(far, f32), C.c_int(n),
-                              ptr(bg), C.c_int(image_width), ptr(out["rgb"]), ptr(out["depth"]), ptr(out["alpha"]),
-                              ptr(out["counter"]), ptr(workspace), C.c_size_t(workspace.numel() * workspace.element_size()),
-                              ptr(stats), stream()))
+    _lib.count(3); call("ia_render_fwd", *args, STREAM)
     return out
 
 
@@ -331,8 +318,7 @@ def deform_query(scene: Scene, pts, eval_mode=True, want_xc=False, stats=None):
     xc = torch.empty((n, 3), device=dev, dtype=f32) if want_xc else None
     best = torch.empty(n, device=dev, dtype=torch.int8) if want_xc else None
     s = scene.c_struct()
-    _lib.count(1); check(lib().ia_deform_query(C.byref(s), ptr(pts, f32), C.c_int(n), C.c_int(1 if eval_mode else 0), ptr(rgb), ptr(sigma),
-                                ptr(xc), ptr(best), ptr(stats), stream()))
+    _lib.count(1); call("ia_deform_query", C.byref(s), pts, n, 1 if eval_mode else 0, rgb, sigma, xc, best, stats, STREAM)
     return (rgb, sigma, xc, best) if want_xc else (rgb, sigma)
 
 
@@ -344,7 +330,7 @@ def broyden(scene: Scene, xd, want_jinv=False):
     xc = torch.empty((n, 13, 3), device=dev, dtype=f32); valid = torch.empty((n, 13), device=dev, dtype=torch.uint8)
     jinv = torch.empty((n, 13, 3, 3), device=dev, dtype=f32) if want_jinv else None
     s = scene.c_struct()
-    _lib.count(1); check(lib().ia_broyden(C.byref(s), ptr(xd, f32), C.c_int(n), ptr(xc), ptr(valid), ptr(jinv), stream()))
+    _lib.count(1); call("ia_broyden", C.byref(s), xd, n, xc, valid, jinv, STREAM)
     return xc, valid.bool(), jinv
 
 
@@ -354,7 +340,7 @@ def ngp_forward(scene: Scene, x):
     n = x.shape[0]
     sigma = torch.empty(n, device=x.device, dtype=f32); rgb = torch.empty((n, 3), device=x.device, dtype=f32)
     s = scene.c_struct()
-    _lib.count(1); check(lib().ia_ngp_forward(C.byref(s), ptr(x, f32), C.c_int(n), ptr(sigma), ptr(rgb), stream()))
+    _lib.count(1); call("ia_ngp_forward", C.byref(s), x, n, sigma, rgb, STREAM)
     return rgb, sigma
 
 
@@ -376,11 +362,10 @@ def train_fwd(scene: Scene, rays_o, rays_d, near, far, bg=None, jitter=None, noi
     key = (dev, n)
     ws = _train_ws.get(key)
     if ws is None:   # kept for the life of the process: a captured CUDA graph may reference it
-        ws = _train_ws[key] = torch.empty(64 + n * S, device=dev, dtype=torch.int32)
-    _lib.count(3); check(lib().ia_train_fwd_split(C.byref(s), ptr(rays_o, f32), ptr(rays_d, f32), ptr(near, f32), ptr(far, f32), C.c_int(n),
-                                                  ptr(bg), ptr(jitter), ptr(noise), ptr(out["rgb"]), ptr(out["depth"]), ptr(out["alpha"]),
-                                                  ptr(out["weights"]), ptr(saved["sigma"]), ptr(saved["rgb"]), ptr(saved["xc"]), ptr(saved["z"]),
-                                                  ptr(saved["count"]), ptr(saved["best"]), ptr(ws), C.c_size_t(ws.numel() * 4), ptr(stats), stream()))
+        ws = _train_ws[key] = torch.empty(call("ia_train_fwd_workspace_bytes", n), device=dev, dtype=torch.uint8)
+    _lib.count(3); call("ia_train_fwd_split", C.byref(s), rays_o, rays_d, near, far, n, bg, jitter, noise, out["rgb"], out["depth"],
+                        out["alpha"], out["weights"], saved["sigma"], saved["rgb"], saved["xc"], saved["z"], saved["count"],
+                        saved["best"], ws, ws.numel(), stats, STREAM)
     return out, saved
 
 
@@ -396,11 +381,10 @@ def composite_bwd(near, far, bg, noise, saved, g_rgb=None, g_depth=None, g_alpha
     g_rgb, g_depth, g_alpha, g_weights = c(g_rgb), c(g_depth), c(g_alpha), c(g_weights)
     l_xd = torch.empty((cap, 3), device=dev, dtype=f32) if rays is not None else None
     l_best = torch.empty(cap, device=dev, dtype=torch.int8) if rays is not None else None
-    _lib.count(1); check(lib().ia_composite_bwd(C.c_int(n), ptr(near, f32), ptr(far, f32), ptr(bg), ptr(noise), ptr(saved["sigma"]),
-                                                ptr(saved["rgb"]), ptr(saved["xc"]), ptr(saved["z"]), ptr(saved["count"]), ptr(saved["best"]),
-                                                ptr(g_rgb), ptr(g_depth), ptr(g_alpha), ptr(g_weights), ptr(l_xc), ptr(l_ds), ptr(l_dc),
-                                                ptr(l_count), ptr(rays[0]) if rays is not None else None,
-                                                ptr(rays[1]) if rays is not None else None, ptr(l_xd), ptr(l_best), stream()))
+    rays_o, rays_d = rays if rays is not None else (None, None)
+    _lib.count(1); call("ia_composite_bwd", n, near, far, bg, noise, saved["sigma"], saved["rgb"], saved["xc"], saved["z"], saved["count"],
+                        saved["best"], g_rgb, g_depth, g_alpha, g_weights, l_xc, l_ds, l_dc, l_count, rays_o, rays_d, l_xd, l_best,
+                        STREAM)
     if rays is not None:
         return l_xc, l_ds, l_dc, l_count, l_xd, l_best
     return l_xc, l_ds, l_dc, l_count
@@ -413,77 +397,74 @@ def ngp_backward(scene: Scene, xc, dsigma, drgb, count, grad_enc, grad_col, grad
     """accumulate d loss / d (encoder.params, color_net.params) for a list of canonical points"""
     cap = xc.shape[0]
     dev = xc.device
-    nbytes = int(lib().ia_ngp_backward_scratch_bytes(C.c_int(cap)))
+    nbytes = call("ia_ngp_backward_scratch_bytes", cap)
     key = (dev.index, )
     if key not in _SCRATCH or _SCRATCH[key].numel() < nbytes:
         _SCRATCH[key] = torch.empty(nbytes, device=dev, dtype=torch.uint8)
     s = scene.c_struct()
-    _lib.count(2); check(lib().ia_ngp_backward(C.byref(s), ptr(xc, f32), ptr(dsigma, f32), ptr(drgb, f32), ptr(count), C.c_int(cap),
-                                               C.c_float(grad_scale), ptr(grad_enc, f32), ptr(grad_col, f32), ptr(_SCRATCH[key]),
-                                               ptr(denc_out), stream()))
+    _lib.count(2); call("ia_ngp_backward", C.byref(s), xc, dsigma, drgb, count, cap, grad_scale, grad_enc, grad_col, _SCRATCH[key],
+                        denc_out, STREAM)
 
 
 def adam_step(params, grads, exp_avg, exp_avg_sq, lr, betas, eps, step, inv_grad_scale=1.0, found_inf=None, grad_scale_dev=None):
-    _lib.count(1); check(lib().ia_adam_step(ptr(params, f32), ptr(grads, f32), ptr(exp_avg, f32), ptr(exp_avg_sq, f32),
-                                            C.c_long(params.numel()), C.c_float(lr), C.c_float(betas[0]), C.c_float(betas[1]),
-                                            C.c_float(eps), C.c_int(step), C.c_float(inv_grad_scale), ptr(grad_scale_dev), ptr(found_inf), stream()))
+    _lib.count(1); call("ia_adam_step", params, grads, exp_avg, exp_avg_sq, params.numel(), lr, betas[0], betas[1], eps, step,
+                        inv_grad_scale, grad_scale_dev, found_inf, STREAM)
 
 
 def grad_check_finite(grads, found_inf):
-    _lib.count(1); check(lib().ia_grad_check_finite(ptr(grads, f32), C.c_long(grads.numel()), ptr(found_inf, f32), stream()))
+    _lib.count(1); call("ia_grad_check_finite", grads, grads.numel(), found_inf, STREAM)
 
 
 def adam_prepare(state, inv_world=1.0, grad_scale_dev=None, found_inf=None):
-    _lib.count(1); check(lib().ia_adam_prepare(ptr(state, f32), C.c_float(inv_world), ptr(grad_scale_dev), ptr(found_inf), stream()))
+    _lib.count(1); call("ia_adam_prepare", state, inv_world, grad_scale_dev, found_inf, STREAM)
 
 
 def adam_step_dev(params, grads, exp_avg, exp_avg_sq, state, found_inf=None, half_out=None, half_skip=0):
-    _lib.count(1); check(lib().ia_adam_step_dev(ptr(params, f32), ptr(grads, f32), ptr(exp_avg, f32), ptr(exp_avg_sq, f32),
-                                                C.c_long(params.numel()), ptr(state, f32), ptr(found_inf), ptr(half_out),
-                                                C.c_long(half_skip), stream()))
+    _lib.count(1); call("ia_adam_step_dev", params, grads, exp_avg, exp_avg_sq, params.numel(), state, found_inf, half_out, half_skip,
+                        STREAM)
+
+
+def _fp16(t):
+    """the header declares fp16 inputs as void*, so their dtype is checked here"""
+    if t.dtype != torch.float16:
+        raise RuntimeError(f"expected {torch.float16}, got {t.dtype}")
+    return t
 
 
 def mlp_to_half_from_half(enc_mlp_h, col_h, mlp_h):
-    _lib.count(1); check(lib().ia_mlp_to_half_from_half(ptr(enc_mlp_h, torch.float16), ptr(col_h, torch.float16), ptr(mlp_h), stream()))
+    _lib.count(1); call("ia_mlp_to_half_from_half", _fp16(enc_mlp_h), _fp16(col_h), mlp_h, STREAM)
 
 
 def grad_poison_shards(grads, shard_elems: int, n_shards: int, found_inf):
-    _lib.count(1); check(lib().ia_grad_poison_shards(ptr(grads, f32), C.c_long(shard_elems), C.c_int(n_shards), ptr(found_inf, f32), stream()))
+    _lib.count(1); call("ia_grad_poison_shards", grads, shard_elems, n_shards, found_inf, STREAM)
 
 
 def peer_reduce_check(peer_grads_dev: int, n_peers: int, shard_off: int, shard_sum, peer_flags_dev: int, rank: int, found_in=None):
-    _lib.count(1); check(lib().ia_peer_reduce_check(C.c_void_p(int(peer_grads_dev)), C.c_int(n_peers), C.c_long(shard_off), C.c_long(shard_sum.numel()),
-                                                    ptr(shard_sum, f32), C.c_void_p(int(peer_flags_dev)), C.c_int(rank), ptr(found_in), stream()))
+    _lib.count(1); call("ia_peer_reduce_check", int(peer_grads_dev), n_peers, shard_off, shard_sum.numel(), shard_sum, int(peer_flags_dev),
+                        rank, found_in, STREAM)
 
 
 def peer_flags_to_found(flags, n_peers: int, found_inf):
-    _lib.count(1); check(lib().ia_peer_flags_to_found(ptr(flags, f32), C.c_int(n_peers), ptr(found_inf, f32), stream()))
+    _lib.count(1); call("ia_peer_flags_to_found", flags, n_peers, found_inf, STREAM)
 
 
 def adam_step_dev_peer(params, grads, exp_avg, exp_avg_sq, state, found_inf, peer_half_dev: int, n_peers: int, shard_off: int):
-    _lib.count(1); check(lib().ia_adam_step_dev_peer(ptr(params, f32), ptr(grads, f32), ptr(exp_avg, f32), ptr(exp_avg_sq, f32),
-                                                     C.c_long(params.numel()), ptr(state, f32), ptr(found_inf), C.c_void_p(int(peer_half_dev)),
-                                                     C.c_int(n_peers), C.c_long(shard_off), stream()))
+    _lib.count(1); call("ia_adam_step_dev_peer", params, grads, exp_avg, exp_avg_sq, params.numel(), state, found_inf,
+                        int(peer_half_dev), n_peers, shard_off, STREAM)
 
 
 def mlp_to_half(enc_params, col_params, mlp_h):
-    _lib.count(1); check(lib().ia_mlp_to_half(ptr(enc_params, f32), ptr(col_params, f32), ptr(mlp_h), stream()))
+    _lib.count(1); call("ia_mlp_to_half", enc_params, col_params, mlp_h, STREAM)
 
 
 # ------------------------------------------------------------------------------------------------------------------
 # legacy kernel-for-kernel operators (raymarch_kernel.* of the reference, renderers/cuda/raymarcher.cpp:77-81)
 # ------------------------------------------------------------------------------------------------------------------
-def _grid_u8(density_grid):
-    g = density_grid.contiguous()
-    return g.view(torch.uint8) if g.dtype == torch.bool else g
-
-
 def raymarch_train(rays_o, rays_d, nears, fars, density_grid, scale, offset, step_size, N_steps):
     n = rays_o.shape[0]
     depths = torch.zeros((n, N_steps), device=rays_o.device, dtype=f32)
-    _lib.count(1); check(lib().ia_raymarch_train(ptr(rays_o, f32), ptr(rays_d, f32), ptr(nears, f32), ptr(fars, f32), C.c_int(n),
-                                                 ptr(_grid_u8(density_grid)), C.c_int(density_grid.shape[0]), ptr(scale, f32), ptr(offset, f32),
-                                                 ptr(step_size, f32), C.c_int(N_steps), ptr(depths), stream()))
+    _lib.count(1); call("ia_raymarch_train", rays_o, rays_d, nears, fars, n, density_grid.contiguous(), density_grid.shape[0], scale,
+                        offset, step_size, N_steps, depths, STREAM)
     return depths
 
 
@@ -493,18 +474,20 @@ def raymarch_test(rays_o, rays_d, nears, fars, alives, density_grid, scale, offs
     dev = rays_o.device
     pts = torch.zeros((a, N_steps, 3), device=dev, dtype=f32); deltas = torch.zeros((a, N_steps), device=dev, dtype=f32)
     depths = torch.zeros((a, N_steps), device=dev, dtype=f32)
-    _lib.count(1); check(lib().ia_raymarch_test(ptr(rays_o, f32), ptr(rays_d, f32), ptr(nears, f32), ptr(fars, f32), ptr(alives, torch.int64),
-                                                C.c_int(a), ptr(_grid_u8(density_grid)), C.c_int(density_grid.shape[0]), ptr(scale, f32),
-                                                ptr(offset, f32), ptr(step_size, f32), C.c_int(N_steps), ptr(pts), ptr(deltas), ptr(depths), stream()))
+    _lib.count(1); call("ia_raymarch_test", rays_o, rays_d, nears, fars, alives, a, density_grid.contiguous(), density_grid.shape[0],
+                        scale, offset, step_size, N_steps, pts, deltas, depths, STREAM)
     return [pts, deltas, depths]
 
 
 def composite_test(rgb_vals, sigma_vals, delta_vals, depth_vals, alive_indices, color, depth, no_hit, thresh):
     a = alive_indices.shape[0]
     n_steps = sigma_vals.shape[1] if a else 0
-    _lib.count(1); check(lib().ia_composite_test(ptr(rgb_vals.contiguous(), f32), ptr(sigma_vals.contiguous(), f32), ptr(delta_vals, f32),
-                                                 ptr(depth_vals, f32), ptr(alive_indices, torch.int64), C.c_int(a), C.c_int(n_steps),
-                                                 ptr(color, f32), ptr(depth, f32), ptr(no_hit, f32), C.c_float(thresh), stream()))
+    _lib.count(1); call("ia_composite_test", rgb_vals.contiguous(), sigma_vals.contiguous(), delta_vals, depth_vals, alive_indices, a,
+                        n_steps, color, depth, no_hit, thresh, STREAM)
+
+
+def _flat(t):
+    return t.reshape(-1).contiguous() if t is not None else None
 
 
 def smpl_tfs(global_orient, body_pose, transl, joints, parents_i32, tfs_inv_t, want_A=False):
@@ -512,10 +495,8 @@ def smpl_tfs(global_orient, body_pose, transl, joints, parents_i32, tfs_inv_t, w
     dev = body_pose.device
     tfs = torch.empty((1, 24, 4, 4), device=dev, dtype=f32); w2s = torch.empty((1, 4, 4), device=dev, dtype=f32)
     A = torch.empty((1, 24, 4, 4), device=dev, dtype=f32) if want_A else None
-    _lib.count(1); check(lib().ia_smpl_tfs(ptr(global_orient.reshape(-1).contiguous(), f32), ptr(body_pose.reshape(-1).contiguous(), f32),
-                                           ptr(transl.reshape(-1).contiguous(), f32) if transl is not None else None,
-                                           ptr(joints.reshape(-1).contiguous(), f32), ptr(parents_i32, torch.int32),
-                                           ptr(tfs_inv_t.reshape(-1).contiguous(), f32), ptr(tfs), ptr(w2s), ptr(A), stream()))
+    _lib.count(1); call("ia_smpl_tfs", _flat(global_orient), _flat(body_pose), _flat(transl), _flat(joints), parents_i32,
+                        _flat(tfs_inv_t), tfs, w2s, A, STREAM)
     return tfs, w2s, A
 
 
@@ -526,9 +507,7 @@ def transform_rays(w2s, rays_o, rays_d, index=None):
     n = o.shape[0] if index is None else index.numel()
     o2 = torch.empty((n, 3), device=o.device, dtype=f32); d2 = torch.empty((n, 3), device=o.device, dtype=f32)
     near = torch.empty(n, device=o.device, dtype=f32); far = torch.empty(n, device=o.device, dtype=f32)
-    _lib.count(1); check(lib().ia_transform_rays(ptr(w2s.reshape(-1, 4, 4)[0].float().contiguous(), f32), ptr(o, f32), ptr(d, f32),
-                                                 ptr(index, torch.int32) if index is not None else None, C.c_int(n),
-                                                 ptr(o2), ptr(d2), ptr(near), ptr(far), stream()))
+    _lib.count(1); call("ia_transform_rays", w2s.reshape(-1, 4, 4)[0].float().contiguous(), o, d, index, n, o2, d2, near, far, STREAM)
     return o2, d2, near, far
 
 
@@ -539,10 +518,8 @@ def nerf_loss(out: dict, target_rgb, target_alpha, w_rgb=1.0, w_alpha=0.1, w_reg
     dev = out["rgb"].device
     g_rgb = torch.empty_like(out["rgb"]); g_alpha = torch.empty_like(out["alpha"]); g_w = torch.empty_like(out["weights"])
     sums = torch.empty(12, device=dev, dtype=f32)
-    _lib.count(1); check(lib().ia_nerf_loss(C.c_int(n), C.c_int(S), ptr(out["rgb"], f32), ptr(out["alpha"], f32), ptr(out["weights"], f32),
-                                            ptr(target_rgb.reshape(-1, 3).contiguous(), f32), ptr(target_alpha.reshape(-1).contiguous(), f32),
-                                            C.c_float(w_rgb), C.c_float(w_alpha), C.c_float(w_reg), ptr(scale_dev), ptr(g_rgb), ptr(g_alpha),
-                                            ptr(g_w), ptr(sums), stream()))
+    _lib.count(1); call("ia_nerf_loss", n, S, out["rgb"], out["alpha"], out["weights"], target_rgb.reshape(-1, 3).contiguous(),
+                        _flat(target_alpha), w_rgb, w_alpha, w_reg, scale_dev, g_rgb, g_alpha, g_w, sums, STREAM)
     # the loss terms are finished inside the kernel (views of its output: no torch launches)
     losses = {"mse_loss": sums[4], "loss_alpha_coarse": sums[5], "reg_alpha": sums[6], "reg_density": sums[7], "loss": sums[8]}
     return losses, g_rgb, g_alpha, g_w
@@ -560,11 +537,9 @@ def ngp_loss(out: dict, target_rgb, target_alpha, patch_rays: int, w_rgb=1.0, w_
     g_w = torch.empty_like(out["weights"])
     sums = torch.empty(16, device=dev, dtype=f32)
     extra = g_rgb_extra.reshape(-1, 3).contiguous() if g_rgb_extra is not None else None
-    _lib.count(1); check(lib().ia_ngp_loss(C.c_int(n), C.c_int(S), C.c_int(patch_rays), ptr(out["rgb"], f32), ptr(out["alpha"], f32),
-                                           ptr(out["depth"], f32), ptr(out["weights"], f32),
-                                           ptr(target_rgb.reshape(-1, 3).contiguous(), f32), ptr(target_alpha.reshape(-1).contiguous(), f32),
-                                           C.c_float(w_rgb), C.c_float(w_alpha), C.c_float(w_reg), C.c_float(w_depth_reg), ptr(extra, f32),
-                                           ptr(scale_dev), ptr(g_rgb), ptr(g_alpha), ptr(g_depth), ptr(g_w), ptr(sums), stream()))
+    _lib.count(1); call("ia_ngp_loss", n, S, patch_rays, out["rgb"], out["alpha"], out["depth"], out["weights"],
+                        target_rgb.reshape(-1, 3).contiguous(), _flat(target_alpha), w_rgb, w_alpha, w_reg, w_depth_reg, extra, scale_dev,
+                        g_rgb, g_alpha, g_depth, g_w, sums, STREAM)
     losses = {"mse_loss": sums[4], "loss_alpha_coarse": sums[5], "reg_alpha": sums[6], "reg_density": sums[7],
               "loss_depth_reg": sums[10], "loss": sums[12]}
     return losses, g_rgb, g_alpha, g_depth, g_w
@@ -572,8 +547,8 @@ def ngp_loss(out: dict, target_rgb, target_alpha, patch_rays: int, w_rgb=1.0, w_
 
 def pose_grad(scene: Scene, lbs_voxel, xd, best, denc, count, grad_tfs):
     """d loss / d tfs (+=) by implicit differentiation of the Broyden roots (deformer_torch.py:50-67)"""
-    _lib.count(1); check(lib().ia_pose_grad(C.byref(scene.c_struct()), ptr(lbs_voxel.reshape(24, -1).contiguous(), f32), ptr(xd, f32),
-                                            ptr(best, torch.int8), ptr(denc, f32), ptr(count), C.c_int(xd.shape[0]), ptr(grad_tfs, f32), stream()))
+    _lib.count(1); call("ia_pose_grad", C.byref(scene.c_struct()), lbs_voxel.reshape(24, -1).contiguous(), xd, best, denc, count,
+                        xd.shape[0], grad_tfs, STREAM)
 
 
 def skin_points(lbs_voxel, offset_k, scale_k, tfs, xc, want_weights=False):
@@ -586,9 +561,8 @@ def skin_points(lbs_voxel, offset_k, scale_k, tfs, xc, want_weights=False):
     F, n = tfs.shape[0], xc.shape[0]
     xd = torch.empty((F, n, 3), device=xc.device, dtype=f32)
     weights = torch.empty((n, 24), device=xc.device, dtype=f32) if want_weights else None
-    _lib.count(1); check(lib().ia_skin_points(ptr(lbs_voxel.reshape(24, D, H, W).contiguous(), f32), C.c_int(D), C.c_int(H), C.c_int(W),
-                                              ptr(offset_k.reshape(3).contiguous(), f32), ptr(scale_k.reshape(3).contiguous(), f32),
-                                              ptr(tfs, f32), C.c_int(F), ptr(xc, f32), C.c_int(n), ptr(xd), ptr(weights), stream()))
+    _lib.count(1); call("ia_skin_points", lbs_voxel.reshape(24, D, H, W).contiguous(), D, H, W, offset_k.reshape(3).contiguous(),
+                        scale_k.reshape(3).contiguous(), tfs, F, xc, n, xd, weights, STREAM)
     return (xd, weights) if want_weights else xd
 
 
@@ -608,10 +582,8 @@ def vertex_skin_weights(lbs_voxel, offset_k, scale_k, xc, K: int = 4, want_dropp
     weights = torch.empty((n, K), device=dev, dtype=f32)
     dropped = torch.empty(n, device=dev, dtype=f32) if want_dropped else None
     n_fallback = torch.zeros(1, device=dev, dtype=torch.int32)
-    _lib.count(1); check(lib().ia_vertex_skin_weights(ptr(lbs_voxel.reshape(24, D, H, W).contiguous(), f32), C.c_int(D), C.c_int(H),
-                                                      C.c_int(W), ptr(offset_k.reshape(3).contiguous(), f32),
-                                                      ptr(scale_k.reshape(3).contiguous(), f32), ptr(xc, f32), C.c_int(n), C.c_int(K),
-                                                      ptr(joints), ptr(weights), ptr(dropped), ptr(n_fallback, torch.int32), stream()))
+    _lib.count(1); call("ia_vertex_skin_weights", lbs_voxel.reshape(24, D, H, W).contiguous(), D, H, W, offset_k.reshape(3).contiguous(),
+                        scale_k.reshape(3).contiguous(), xc, n, K, joints, weights, dropped, n_fallback, STREAM)
     return (joints, weights, n_fallback, dropped) if want_dropped else (joints, weights, n_fallback)
 
 
@@ -636,9 +608,8 @@ def nv_pose_grad(scene: Scene, rays_o, rays_d, l_rz, best, denc, count, grad_tab
     """d loss / d nearest-vertex table [V,12] and, when given, d loss / d rays_o / rays_d [n,3] (all +=) for a
     compositing-backward list whose l_xd was produced with ray_slot_codes (ia_nv_pose_grad)"""
     n = rays_o.numel() // 3
-    _lib.count(1); check(lib().ia_nv_pose_grad(C.byref(scene.c_struct()), ptr(rays_o, f32), ptr(rays_d, f32), C.c_int(n), ptr(l_rz, f32),
-                                               ptr(best, torch.int8), ptr(denc, f32), ptr(count), C.c_int(l_rz.shape[0]),
-                                               ptr(grad_table, f32), ptr(grad_rays_o, f32), ptr(grad_rays_d, f32), stream()))
+    _lib.count(1); call("ia_nv_pose_grad", C.byref(scene.c_struct()), rays_o, rays_d, n, l_rz, best, denc, count, l_rz.shape[0],
+                        grad_table, grad_rays_o, grad_rays_d, STREAM)
 
 
 def voxelize_weights(verts, vert_weights, xs, ys, zs, offset, scale, ratio, knn=30, smooth_passes=30):
@@ -648,11 +619,10 @@ def voxelize_weights(verts, vert_weights, xs, ys, zs, offset, scale, ratio, knn=
     out = torch.empty((1, 24, D, H, W), device=dev, dtype=f32)
     scratch = torch.empty_like(out) if smooth_passes > 0 else None
     _lib.count(1 + smooth_passes)
-    check(lib().ia_voxelize_weights(ptr(verts.reshape(-1, 3).contiguous(), f32), ptr(vert_weights.reshape(-1, 24).contiguous(), f32),
-                                    C.c_int(verts.reshape(-1, 3).shape[0]), ptr(xs.contiguous(), f32), ptr(ys.contiguous(), f32),
-                                    ptr(zs.contiguous(), f32), C.c_int(D), C.c_int(H), C.c_int(W), ptr(offset.reshape(3).contiguous(), f32),
-                                    ptr(scale.reshape(1).contiguous(), f32), C.c_float(ratio), C.c_int(knn), C.c_int(smooth_passes),
-                                    ptr(out), ptr(scratch), stream()))
+    verts = verts.reshape(-1, 3).contiguous()
+    call("ia_voxelize_weights", verts, vert_weights.reshape(-1, 24).contiguous(), verts.shape[0], xs.contiguous(), ys.contiguous(),
+         zs.contiguous(), D, H, W, offset.reshape(3).contiguous(), scale.reshape(1).contiguous(), ratio, knn, smooth_passes, out,
+         scratch, STREAM)
     return out
 
 
@@ -661,7 +631,7 @@ def ngp_input_grad(scene: Scene, x, denc):
     x = x.reshape(-1, 3).contiguous()
     dx = torch.empty_like(x, dtype=f32)
     s = scene.c_struct()
-    _lib.count(1); check(lib().ia_ngp_input_grad(C.byref(s), ptr(x, f32), ptr(denc, f32), C.c_int(x.shape[0]), ptr(dx), stream()))
+    _lib.count(1); call("ia_ngp_input_grad", C.byref(s), x, denc, x.shape[0], dx, STREAM)
     return dx
 
 
@@ -669,11 +639,8 @@ def smpl_tfs_backward(global_orient, body_pose, transl, joints, parents_i32, tfs
     """reverse mode of smpl_tfs -> (grad_global_orient [1,3], grad_body_pose [1,69], grad_transl [1,3])"""
     dev = body_pose.device
     g_o = torch.empty((1, 3), device=dev, dtype=f32); g_p = torch.empty((1, 69), device=dev, dtype=f32); g_t = torch.empty((1, 3), device=dev, dtype=f32)
-    _lib.count(1); check(lib().ia_smpl_tfs_backward(ptr(global_orient.reshape(-1).contiguous(), f32), ptr(body_pose.reshape(-1).contiguous(), f32),
-                                                    ptr(transl.reshape(-1).contiguous(), f32) if transl is not None else None,
-                                                    ptr(joints.reshape(-1).contiguous(), f32), ptr(parents_i32, torch.int32),
-                                                    ptr(tfs_inv_t.reshape(-1).contiguous(), f32), ptr(grad_tfs.reshape(-1).contiguous(), f32),
-                                                    ptr(g_o), ptr(g_p), ptr(g_t), stream()))
+    _lib.count(1); call("ia_smpl_tfs_backward", _flat(global_orient), _flat(body_pose), _flat(transl), _flat(joints), parents_i32,
+                        _flat(tfs_inv_t), _flat(grad_tfs), g_o, g_p, g_t, STREAM)
     return g_o, g_p, g_t
 
 
@@ -682,8 +649,7 @@ def knn1(pts, verts):
     pts = pts.reshape(-1, 3).contiguous(); verts = verts.reshape(-1, 3).contiguous()
     n = pts.shape[0]
     idx = torch.empty(n, device=pts.device, dtype=torch.int32); d2 = torch.empty(n, device=pts.device, dtype=f32)
-    _lib.count(1); check(lib().ia_knn1(ptr(pts, f32), C.c_int(n), ptr(verts, f32), C.c_int(verts.shape[0]), ptr(idx, torch.int32), ptr(d2),
-                                       stream()))
+    _lib.count(1); call("ia_knn1", pts, n, verts, verts.shape[0], idx, d2, STREAM)
     return d2, idx.long()
 
 
@@ -691,7 +657,7 @@ def knn1(pts, verts):
 # the two tiny-cuda-nn modules as separate operators (bound by the in-repo `tinycudann` module)
 # ------------------------------------------------------------------------------------------------------------------
 def _tcnn_scratch(n, dev):
-    nbytes = int(lib().ia_tcnn_backward_scratch_bytes(C.c_int(n)))
+    nbytes = call("ia_tcnn_backward_scratch_bytes", n)
     key = ("tcnn", dev.index)
     if key not in _SCRATCH or _SCRATCH[key].numel() < nbytes:
         _SCRATCH[key] = torch.empty(nbytes, device=dev, dtype=torch.uint8)
@@ -701,7 +667,7 @@ def _tcnn_scratch(n, dev):
 def tcnn_encoder_forward(scene: Scene, x01):
     x01 = x01.reshape(-1, 3).float().contiguous()
     out = torch.empty((x01.shape[0], 16), device=x01.device, dtype=torch.float16)
-    _lib.count(1); check(lib().ia_tcnn_encoder_forward(C.byref(scene.c_struct()), ptr(x01, f32), C.c_int(x01.shape[0]), ptr(out), stream()))
+    _lib.count(1); call("ia_tcnn_encoder_forward", C.byref(scene.c_struct()), x01, x01.shape[0], out, STREAM)
     return out
 
 
@@ -710,15 +676,15 @@ def tcnn_encoder_backward(scene: Scene, x01, dout16, grad_enc=None, want_denc=Fa
     n, dev = x01.shape[0], x01.device
     denc = torch.empty((n, 32), device=dev, dtype=f32) if want_denc else None
     dummy = torch.zeros(_lib.IA_COL_MLP_PARAMS, device=dev, dtype=f32) if grad_enc is not None else None
-    _lib.count(3); check(lib().ia_tcnn_encoder_backward(C.byref(scene.c_struct()), ptr(x01, f32), ptr(dout16, f32), C.c_int(n), C.c_float(grad_scale),
-                                                        ptr(grad_enc, f32), ptr(dummy), ptr(_tcnn_scratch(n, dev)), ptr(denc), stream()))
+    _lib.count(3); call("ia_tcnn_encoder_backward", C.byref(scene.c_struct()), x01, dout16, n, grad_scale, grad_enc, dummy,
+                        _tcnn_scratch(n, dev), denc, STREAM)
     return denc
 
 
 def tcnn_mlp_forward(mlp_h, in15):
     in15 = in15.reshape(-1, 15).float().contiguous()
     out = torch.empty((in15.shape[0], 3), device=in15.device, dtype=torch.float16)
-    _lib.count(1); check(lib().ia_tcnn_mlp_forward(ptr(mlp_h, torch.float16), ptr(in15, f32), C.c_int(in15.shape[0]), ptr(out), stream()))
+    _lib.count(1); call("ia_tcnn_mlp_forward", _fp16(mlp_h), in15, in15.shape[0], out, STREAM)
     return out
 
 
@@ -727,13 +693,13 @@ def tcnn_mlp_backward(mlp_h, in15, dout3, grad_col=None, want_din=False, grad_sc
     n, dev = in15.shape[0], in15.device
     din = torch.zeros((n, 15), device=dev, dtype=f32) if want_din else None
     dummy = torch.zeros(_lib.IA_ENC_MLP_PARAMS, device=dev, dtype=f32) if grad_col is not None else None
-    _lib.count(3); check(lib().ia_tcnn_mlp_backward(ptr(mlp_h, torch.float16), ptr(in15, f32), ptr(dout3, f32), C.c_int(n), C.c_float(grad_scale),
-                                                    ptr(grad_col, f32), ptr(dummy), ptr(_tcnn_scratch(n, dev)), ptr(din), stream()))
+    _lib.count(3); call("ia_tcnn_mlp_backward", _fp16(mlp_h), in15, dout3, n, grad_scale, grad_col, dummy, _tcnn_scratch(n, dev), din,
+                        STREAM)
     return din
 
 
 def frame_index_bytes(F: int, H: int, W: int, patch: int = 0) -> int:
-    nbytes = int(lib().ia_frame_index_bytes(C.c_int(F), C.c_int(H), C.c_int(W), C.c_int(patch)))
+    nbytes = call("ia_frame_index_bytes", F, H, W, patch)
     if nbytes == 0 and F > 0:
         raise ValueError(f"no frame index for F={F}, H={H}, W={W}, patch={patch}")
     return nbytes
@@ -745,9 +711,8 @@ def frame_index_build(masks, edge_kernel: int = 0, patch: int = 0, dilate: int =
     F, H, W = masks.shape
     index = torch.empty(frame_index_bytes(F, H, W, patch), device=masks.device, dtype=torch.uint8)
     counts = torch.zeros((F, 3), device=masks.device, dtype=torch.int64)
-    _lib.count(2); check(lib().ia_frame_index_build(ptr(masks.contiguous(), f32), C.c_int(F), C.c_int(H), C.c_int(W),
-                                                    C.c_int(edge_kernel), C.c_int(patch), C.c_int(dilate), ptr(index),
-                                                    C.c_size_t(index.numel()), ptr(counts), stream()))
+    _lib.count(2); call("ia_frame_index_build", masks.contiguous(), F, H, W, edge_kernel, patch, dilate, index, index.numel(), counts,
+                        STREAM)
     return index, counts
 
 
@@ -757,14 +722,12 @@ def _sample_outputs(n: int, device):
     return o
 
 
-def _sample_ptrs(o):
-    return [ptr(o[k]) for k in ("rgb", "alpha", "rays_o", "rays_d", "bg_color", "near", "far")]
+def _sample_args(o):
+    return [o[k] for k in ("rgb", "alpha", "rays_o", "rays_d", "bg_color", "near", "far")]
 
 
-def _frame_ptrs(frames):
-    F, H, W = frames["masks"].shape
-    return [ptr(frames["images"], torch.uint8), ptr(frames["masks"], f32), ptr(frames["rays_o"], f32), ptr(frames["rays_d"], f32),
-            ptr(frames["near_far"], f32), C.c_int(F), C.c_int(H), C.c_int(W)]
+def _frame_args(frames):
+    return [frames[k] for k in ("images", "masks", "rays_o", "rays_d", "near_far")] + list(frames["masks"].shape)
 
 
 def sample_edge(frames: dict, index, patch: int, frame: int, num_mask: int, num_edge: int, num_rand: int, words=None, bg=None):
@@ -774,9 +737,8 @@ def sample_edge(frames: dict, index, patch: int, frame: int, num_mask: int, num_
     -> dict of rgb, rays_o, rays_d, bg_color [n,3] and alpha, near, far [n]"""
     n = num_mask + num_edge + num_rand
     out = _sample_outputs(n, frames["masks"].device)
-    _lib.count(1); check(lib().ia_sample_edge(*_frame_ptrs(frames), ptr(index), C.c_int(patch), C.c_int(frame), C.c_int(num_mask),
-                                              C.c_int(num_edge), C.c_int(num_rand), ptr(words, torch.int32), ptr(bg, f32),
-                                              *_sample_ptrs(out), stream()))
+    _lib.count(1); call("ia_sample_edge", *_frame_args(frames), index, patch, frame, num_mask, num_edge, num_rand, words, bg,
+                        *_sample_args(out), STREAM)
     return out
 
 
@@ -784,9 +746,8 @@ def sample_patch(frames: dict, index, frame: int, num_patch: int, patch: int, ra
     """PatchSampler.sample + the dataset's compositing (sampler.py:56-82) in one launch: words [1 + 2*num_patch] int32,
     bg [num_patch*P*P, 3] -> dict of [num_patch*P*P, ...] outputs (patch-major) as sample_edge"""
     out = _sample_outputs(num_patch * patch * patch, frames["masks"].device)
-    _lib.count(1); check(lib().ia_sample_patch(*_frame_ptrs(frames), ptr(index), C.c_int(frame), C.c_int(num_patch), C.c_int(patch),
-                                               C.c_double(ratio_mask), ptr(words, torch.int32), ptr(bg, f32), *_sample_ptrs(out),
-                                               stream()))
+    _lib.count(1); call("ia_sample_patch", *_frame_args(frames), index, frame, num_patch, patch, ratio_mask, words, bg,
+                        *_sample_args(out), STREAM)
     return out
 
 
@@ -797,8 +758,7 @@ def test_panel(pred, gt):
         raise ValueError(f"test_panel: pred and gt must both be [F,H,W,3], got {tuple(pred.shape)} and {tuple(gt.shape)}")
     F, H, W, _ = pred.shape
     panel = torch.empty((F, H, 3 * W, 3), device=pred.device, dtype=torch.uint8)
-    _lib.count(1); check(lib().ia_test_panel(ptr(pred.contiguous(), f32), ptr(gt.contiguous(), f32), C.c_int(F), C.c_int(H),
-                                             C.c_int(W), ptr(panel), stream()))
+    _lib.count(1); call("ia_test_panel", pred.contiguous(), gt.contiguous(), F, H, W, panel, STREAM)
     return panel
 
 
@@ -836,9 +796,8 @@ def image_metrics(a, b):
     sse = torch.empty(F, device=a.device, dtype=torch.int64)
     ssim_fx = torch.empty(F, device=a.device, dtype=torch.int64)
     taps = (C.c_double * SSIM_TAPS)(*ssim_taps().tolist())
-    _lib.count(1); check(lib().ia_image_metrics(C.c_void_p(a.data_ptr()), C.c_long(fa), C.c_long(ra), C.c_void_p(b.data_ptr()),
-                                                C.c_long(fb), C.c_long(rb), C.c_int(F), C.c_int(H), C.c_int(W), taps, ptr(sse),
-                                                ptr(ssim_fx), stream()))
+    _lib.count(1); call("ia_image_metrics", C.c_void_p(a.data_ptr()), fa, ra, C.c_void_p(b.data_ptr()), fb, rb, F, H, W, taps, sse, ssim_fx,
+                        STREAM)
     # divisors as tensors: torch divides a CUDA tensor by a Python scalar through its reciprocal, which is not IEEE division
     denom = lambda v: torch.full((F,), float(v), device=a.device, dtype=torch.float64)
     psnr = -10.0 * torch.log10(sse.double() / denom(255.0 ** 2 * (3 * H * W)))
@@ -858,11 +817,9 @@ def gif_quantize(rgba, swap_rb: bool = False):
     palette = torch.empty((F, 256, 3), device=dev, dtype=torch.uint8)
     index = torch.empty((F, H, W), device=dev, dtype=torch.uint8)
     n_colors = torch.empty(F, device=dev, dtype=torch.int32)
-    nbytes = int(lib().ia_gif_quantize_workspace_bytes(C.c_int(F)))
+    nbytes = call("ia_gif_quantize_workspace_bytes", F)
     workspace = torch.empty(nbytes, device=dev, dtype=torch.uint8)
-    _lib.count(3); check(lib().ia_gif_quantize(ptr(rgba), C.c_int(F), C.c_int(H), C.c_int(W), C.c_int(1 if swap_rb else 0),
-                                               ptr(palette), ptr(index), ptr(n_colors, torch.int32), ptr(workspace),
-                                               C.c_size_t(nbytes), stream()))
+    _lib.count(3); call("ia_gif_quantize", rgba, F, H, W, 1 if swap_rb else 0, palette, index, n_colors, workspace, nbytes, STREAM)
     return palette, index, n_colors
 
 
@@ -897,7 +854,7 @@ class SmplFitModel:
 
 
 def smpl_fit_workspace(model: SmplFitModel, F: int) -> torch.Tensor:
-    nbytes = int(lib().ia_smpl_fit_workspace_bytes(C.c_int(model.n_verts), C.c_int(F)))
+    nbytes = call("ia_smpl_fit_workspace_bytes", model.n_verts, F)
     if nbytes == 0:
         raise ValueError(f"smpl_fit: invalid sizes V={model.n_verts} F={F}")
     return torch.empty(nbytes, device=model.v_template.device, dtype=torch.uint8)
@@ -919,8 +876,8 @@ def smpl_fit_forward(model: SmplFitModel, params, F: int, vertex_ids, workspace=
     joints = torch.empty((F, 35, 3), device=dev, dtype=f32)
     A = torch.empty((F, 24, 4, 4), device=dev, dtype=f32)
     s = model.c_struct()
-    _lib.count(6); check(lib().ia_smpl_fit_forward(C.byref(s), ptr(params, f32), C.c_int(F), _int_array(vertex_ids, 11, "vertex_ids"),
-                                                   ptr(workspace), C.c_size_t(workspace.numel()), ptr(verts), ptr(joints), ptr(A), stream()))
+    _lib.count(6); call("ia_smpl_fit_forward", C.byref(s), params, F, _int_array(vertex_ids, 11, "vertex_ids"), workspace,
+                        workspace.numel(), verts, joints, A, STREAM)
     return verts, joints, A
 
 
@@ -937,8 +894,7 @@ def smpl_fit_objective(model: SmplFitModel, params, F: int, keypoints, proj, joi
     fit.proj = C.cast(P, C.c_void_p).value; fit.joint_map = C.cast(jm, C.c_void_p).value
     fit.select = C.cast(sel, C.c_void_p).value; fit.vertex_ids = C.cast(vid, C.c_void_p).value
     fit.threshold = float(threshold)
-    _lib.count(13); check(lib().ia_smpl_fit_objective(C.byref(s), C.byref(fit), ptr(params, f32), C.c_int(F), ptr(workspace),
-                                                      C.c_size_t(workspace.numel()), ptr(loss, f32), ptr(grad, f32), stream()))
+    _lib.count(13); call("ia_smpl_fit_objective", C.byref(s), C.byref(fit), params, F, workspace, workspace.numel(), loss, grad, STREAM)
 
 
 def face_csr(faces, n_verts: int, device):
@@ -955,7 +911,7 @@ def face_csr(faces, n_verts: int, device):
 
 
 def raster_workspace(F: int, n_verts: int, n_faces: int, device) -> torch.Tensor:
-    nbytes = int(lib().ia_raster_workspace_bytes(C.c_int(F), C.c_int(n_verts), C.c_int(n_faces)))
+    nbytes = call("ia_raster_workspace_bytes", F, n_verts, n_faces)
     if nbytes == 0 and F > 0:
         raise ValueError(f"raster: invalid sizes F={F} V={n_verts} NF={n_faces}")
     return torch.empty(max(nbytes, 16), device=device, dtype=torch.uint8)
@@ -982,9 +938,8 @@ def rasterize(verts, faces, K, E, H: int, W: int, workspace=None):
            "depth": torch.empty((F, H, W), device=dev, dtype=f32),
            "bary": torch.empty((F, H, W, 2), device=dev, dtype=f32)}
     Kc, Ec = _camera(K, E)
-    _lib.count(2); check(lib().ia_raster(ptr(verts, f32), C.c_int(F), C.c_int(V), ptr(faces, torch.int32), C.c_int(NF), Kc, Ec,
-                                         C.c_int(H), C.c_int(W), ptr(workspace), C.c_size_t(workspace.numel()),
-                                         ptr(out["face_id"]), ptr(out["depth"]), ptr(out["bary"]), stream()))
+    _lib.count(2); call("ia_raster", verts, F, V, faces, NF, Kc, Ec, H, W, workspace, workspace.numel(), out["face_id"], out["depth"],
+                        out["bary"], STREAM)
     return out
 
 
@@ -998,10 +953,8 @@ def shade_composite(frames, verts, faces, csr, raster: dict, K, E, workspace=Non
     V, NF = verts.shape[1], faces.shape[0]
     workspace = raster_workspace(F, V, NF, verts.device) if workspace is None else workspace
     Kc, Ec = _camera(K, E)
-    _lib.count(2); check(lib().ia_shade_composite(ptr(verts, f32), C.c_int(F), C.c_int(V), ptr(faces, torch.int32), C.c_int(NF),
-                                                  ptr(csr[0], torch.int32), ptr(csr[1], torch.int32), Kc, Ec, C.c_int(H),
-                                                  C.c_int(W), ptr(raster["face_id"], torch.int32), ptr(raster["bary"], f32),
-                                                  ptr(workspace), C.c_size_t(workspace.numel()), ptr(frames), stream()))
+    _lib.count(2); call("ia_shade_composite", verts, F, V, faces, NF, csr[0], csr[1], Kc, Ec, H, W, raster["face_id"], raster["bary"],
+                        workspace, workspace.numel(), frames, STREAM)
     return frames
 
 
@@ -1010,9 +963,7 @@ def vertex_normals(verts, faces, csr):
     (ia_vertex_normals): the normal pass of shade_composite, bit for bit.  One launch."""
     V, NF = verts.shape[0], faces.shape[0]
     normals = torch.empty((V, 3), device=verts.device, dtype=f32)
-    _lib.count(1); check(lib().ia_vertex_normals(ptr(verts.contiguous(), f32), C.c_int(V), ptr(faces.contiguous(), torch.int32),
-                                                 C.c_int(NF), ptr(csr[0], torch.int32), ptr(csr[1], torch.int32), ptr(normals),
-                                                 stream()))
+    _lib.count(1); call("ia_vertex_normals", verts.contiguous(), V, faces.contiguous(), NF, csr[0], csr[1], normals, STREAM)
     return normals
 
 
@@ -1049,14 +1000,12 @@ def mask_largest_component(masks, images=None, images_out=None):
     workspace = None
     for s in range(0, F, chunk):
         n = min(chunk, F - s)
-        nbytes = int(lib().ia_mask_workspace_bytes(C.c_int(n), C.c_int(H), C.c_int(W)))
+        nbytes = call("ia_mask_workspace_bytes", n, H, W)
         if workspace is None or workspace.numel() < nbytes:
             workspace = torch.empty(nbytes, device=dev, dtype=torch.uint8)
         sl = lambda t: None if t is None else t[s:s + n]
-        _lib.count(9); check(lib().ia_mask_largest_component(ptr(sl(masks)), C.c_int(n), C.c_int(H), C.c_int(W),
-                                                             ptr(sl(mask_out)), ptr(sl(images)), ptr(sl(images_out)),
-                                                             ptr(sl(stats), torch.int32), ptr(workspace),
-                                                             C.c_size_t(workspace.numel()), stream()))
+        _lib.count(9); call("ia_mask_largest_component", sl(masks), n, H, W, sl(mask_out), sl(images), sl(images_out), sl(stats), workspace,
+                            workspace.numel(), STREAM)
     return mask_out, images_out, stats
 
 
