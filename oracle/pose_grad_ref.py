@@ -13,6 +13,9 @@
    (Rodrigues with the |r + 1e-8| regularisation, kinematic chain, A + transl, w2s = A_0^-1 by the general inverse of
    snarf_deformer.py:84, tfs = w2s A tfs_inv_t).  `abs_pass=True` runs the same recurrences on absolute values (every
    difference becomes a sum) and returns the per-component magnitude S for the bound k u S.
+ * `nv_contrib32` / `nv_def64` / `nv_bound32`: one list sample of `ia_nv_pose_grad` (nearest-vertex deformer) in float32
+   in the kernel's operation order, its float64 definition on the same posed point and vertex, and the per-sample
+   bound between them; `reduction_bound` bounds a sum of per-entry float atomics.
 """
 from __future__ import annotations
 
@@ -134,6 +137,103 @@ def pose_grad_bound32(jinv, xc, ok, g64, tg64, w64, wabs64, lbs_voxel, offset_k,
     # + the flush of a subnormal contribution to 0 (below 2^-126 per sample)
     return (np.einsum(e, W + Ew, V + Ev, xh) * (1 + gamma(2)) - np.einsum(e, W, V, xh)
             + np.finfo(f32).tiny * (1 if per_sample else len(x)))
+
+
+def flush32(t):
+    """the float atomics' flush of a subnormal term to (sign-preserving) zero"""
+    t = np.array(t, f32)
+    t[np.abs(t) < np.finfo(f32).tiny] = 0
+    return t
+
+
+def reduction_bound(n, mag):
+    """per entry: gamma_n (sum |t| + |prior|) + n 2^-126 for n terms, each its own float atomic, onto the prior (mag =
+    sum |t| + |prior| per entry; no warp or CTA tree, so n is the number of terms that land on the entry)"""
+    n = np.asarray(n, f64)
+    return gamma(n) * np.asarray(mag, f64) + n * np.finfo(f32).tiny
+
+
+# ---------------------------------------------------------------------------------------------------------------------
+# ia_nv_pose_grad (nearest-vertex deformer)
+# ---------------------------------------------------------------------------------------------------------------------
+def nv_point32(rays_o, rays_d, ray, z, verts, table, thr2):
+    """the kernel's per-sample forward of a list sample (ray index, z), in float32 (`-fmad=false`) -> (x [P,3],
+    vertex [P] (-1: none within the threshold, or the ray index outside 0 .. n_rays - 1), d2 [P], x_c [P,3]):
+    x_a = f32(z d_a) + o_a; the vertex is voxelize_ref.knn1 (first minimum: the lower index wins ties), accepted when
+    d2 < thr2; x_c_r = ((T_r0 x_0 + T_r1 x_1) + T_r2 x_2) + T_r3 (nv_apply)"""
+    from . import voxelize_ref
+    O = np.asarray(rays_o, f32).reshape(-1, 3)
+    Dd = np.asarray(rays_d, f32).reshape(-1, 3)
+    ray = np.asarray(ray).reshape(-1).astype(np.int64)
+    z = np.asarray(z, f32).reshape(-1)
+    ok = (ray >= 0) & (ray < len(O))
+    r = np.where(ok, ray, 0)
+    x = (z[:, None] * Dd[r]) + O[r]
+    d2, v = voxelize_ref.knn1(x, verts)
+    thr2 = f32(thr2)
+    v = np.where(ok & (d2 < thr2), v, -1)
+    T = np.asarray(table, f32).reshape(-1, 3, 4)[np.maximum(v, 0)]
+    xc = ((T[:, :, 0] * x[:, 0, None] + T[:, :, 1] * x[:, 1, None]) + T[:, :, 2] * x[:, 2, None]) + T[:, :, 3]
+    xc[v < 0] = 0
+    return x, v, d2, xc
+
+
+def nv_contrib32(rays_o, rays_d, ray, z, verts, table, thr2, g, point=None):
+    """one list sample's float32 contribution to ia_nv_pose_grad, in the kernel's operation order -> dict of
+    table [P,3,4] (row `vertex`), o [P,3], d [P,3] (row `ray`), with x, vertex, x_c of nv_point32 (`point`: its result,
+    if already computed).  g [P,3]: d loss / d x_c by hash_input_grad at x_c (`ops.ngp_input_grad`).
+      table term f32(g_r xh_c), xh = (x, 1), none for g_r = 0;
+      gx_c = ((0 + g_0 T_0c) + g_1 T_1c) + g_2 T_2c, o term gx_c, d term f32(z gx_c);
+    a sample without a vertex or with g = 0 contributes nothing, and every term passes the atomics' subnormal flush."""
+    x, v, d2, xc = point if point is not None else nv_point32(rays_o, rays_d, ray, z, verts, table, thr2)
+    g = np.asarray(g, f32).reshape(-1, 3)
+    z = np.asarray(z, f32).reshape(-1)
+    T = np.asarray(table, f32).reshape(-1, 3, 4)[np.maximum(v, 0)]
+    act = (v >= 0) & (g != 0).any(1)
+    xh = np.concatenate([x, np.ones((len(x), 1), f32)], 1)
+    tt = g[:, :, None] * xh[:, None, :]
+    gx = np.zeros((len(x), 3), f32)
+    for r in range(3):
+        gx = gx + g[:, r, None] * T[:, r, :3]
+    gd = z[:, None] * gx
+    tt[~act], gx[~act], gd[~act] = 0, 0, 0
+    return {"table": flush32(tt), "o": flush32(gx), "d": flush32(gd), "x": x, "vertex": v, "d2": d2, "xc": xc, "active": act}
+
+
+def nv_def64(x, vertex, z, table, g64):
+    """the definition in float64 on the forward's own posed points x [P,3] and vertices (-1: none): the vertex is piecewise
+    constant in x and the search carries no gradient (smpl_deformer.py:94-95), x_c = T_v [x, 1], so
+    d L / d T_v[r][c] = g_r [x, 1]_c, d L / d o = T_v^T g, d L / d d = z T_v^T g, g = g64 (`input_grad64` at x_c).
+    -> dict of table [P,3,4], o [P,3], d [P,3] and their magnitudes (|.| of every product) table_abs, o_abs, d_abs"""
+    v = np.asarray(vertex).reshape(-1)
+    T = np.asarray(table, f64).reshape(-1, 3, 4)[np.maximum(v, 0)]
+    g = np.asarray(g64, f64).reshape(-1, 3) * (v >= 0)[:, None]
+    z = np.asarray(z, f32).astype(f64).reshape(-1)
+    xh = np.concatenate([np.asarray(x, f64).reshape(-1, 3), np.ones((len(v), 1))], 1)
+    o = np.einsum("prc,pr->pc", T[:, :, :3], g)
+    oa = np.einsum("prc,pr->pc", np.abs(T[:, :, :3]), np.abs(g))
+    return {"table": g[:, :, None] * xh[:, None, :], "o": o, "d": z[:, None] * o,
+            "table_abs": np.abs(g)[:, :, None] * np.abs(xh)[:, None, :], "o_abs": oa, "d_abs": np.abs(z)[:, None] * oa}
+
+
+def nv_bound32(x, vertex, z, table, g64, tg64):
+    """per sample, the bound on |nv_contrib32 - nv_def64| from the roundings: g of hash_input_grad within gamma_32 tg of
+    g64 (as for ia_pose_grad), one rounding per product of a table term, gamma_3 on the 3-term dot product T^T g, one
+    more rounding for the z of the d term, and 2^-126 for a term the atomics flush -> dict of table, o, d"""
+    v = np.asarray(vertex).reshape(-1)
+    on = (v >= 0)[:, None]
+    T = np.abs(np.asarray(table, f64).reshape(-1, 3, 4)[np.maximum(v, 0)][:, :, :3])
+    G = np.abs(np.asarray(g64, f64).reshape(-1, 3)) * on
+    Eg = gamma(32) * np.asarray(tg64, f64).reshape(-1, 3) * on
+    az = np.abs(np.asarray(z, f32).astype(f64).reshape(-1))[:, None]
+    xh = np.abs(np.concatenate([np.asarray(x, f64).reshape(-1, 3), np.ones((len(v), 1))], 1))
+    tiny = np.finfo(f32).tiny
+    tab = ((G + Eg) * (1 + gamma(1)) - G)[:, :, None] * xh[:, None, :] + tiny
+    GT = np.einsum("prc,pr->pc", T, G)
+    ET = np.einsum("prc,pr->pc", T, G + Eg)
+    o = (1 + gamma(3)) * ET - GT + tiny
+    d = az * ((1 + gamma(4)) * ET - GT) + tiny
+    return {"table": tab * on[:, :, None], "o": o * on, "d": d * on}
 
 
 def launch_depth(count, capacity, sms):
