@@ -169,6 +169,33 @@ int ia_pack_occupancy(const uint8_t* field_bool, uint32_t* bits, int G, ia_strea
 int ia_occupancy_build(const float* density, int G, uint8_t* field_out, uint32_t* bits_out, void* workspace,
                        size_t workspace_bytes, ia_stream_t stream);
 
+/* demo.yaml's `smpl_init` (DESIGN.md §3.6, §5.13): the first step-< 500 grid update of a training frame seeds its grid
+ * from the posed SMPL mesh (density_grid.py:52-68, kaolin's point_to_mesh_distance and check_sign).
+ *
+ * ia_smpl_init_seed: unless *seeded != 0 (then the field and cache are left as they are), over the cell centres
+ *   c_i = (i / G + 0.5 / G) * ext + lo (float32, per axis; lo, ext from aabb6 = min xyz, max xyz) of a G^3 grid
+ *   (x slowest): field_out[c] = sqrtf(d2) < 0.01f || inside(c), with d2 the float32 squared distance to the nearest of
+ *   the n_faces triangles faces [n_faces][3] (int32 indices into verts [n_verts][3], each in [0, n_verts): the caller
+ *   guarantees it, the kernels do not check) and inside(c) the parity of the
+ *   crossings of the +z ray from c with the triangles (a triangle covers a column when the three edge functions of its
+ *   xy projection, each evaluated in the canonical order of its endpoints, share one sign; a zero edge function takes
+ *   the sign at the point moved by (eps, eps^2)); cache[c] = max(0.8 cache[c], field ? +inf : 0).  Then bits_out
+ *   [G^3/32 + 8] = ia_pack_occupancy(field_out) (unchanged for a seeded frame) and *seeded = 1.  seeded: device int32 [1].
+ *   workspace: device, ia_smpl_init_workspace_bytes(G) bytes.  No host synchronisation.
+ *   IA_EINVAL: G not a multiple of 32 in [32, 1024], n_verts < 1, n_faces < 0, a short workspace, a NULL pointer.
+ * ia_occupancy_frame_copy: f = clamp(*idx, 0, n_frames - 1) (idx: device int64 [1]); store = 0 copies frame f of the
+ *   stacked grids (cache_all [n_frames][G^3] fp32, field_all [n_frames][G^3] bool, bits_all [n_frames][G^3/32 + 8],
+ *   seeded_all [n_frames] int32) into the working grid (cache, field, bits, seeded [1]); store = 1 copies it back.
+ *   cache_all, field_all, cache and field 16-byte aligned.  IA_EINVAL: n_frames < 1, a bad G or store, a NULL pointer,
+ *   a misaligned pointer. */
+size_t ia_smpl_init_workspace_bytes(int G);
+int ia_smpl_init_seed(const float* verts, int n_verts, const int* faces, int n_faces, const float* aabb6, int G,
+                      int32_t* seeded, float* cache, uint8_t* field_out, uint32_t* bits_out, void* workspace,
+                      size_t workspace_bytes, ia_stream_t stream);
+int ia_occupancy_frame_copy(const int64_t* idx, int n_frames, int G, float* cache_all, uint8_t* field_all, uint32_t* bits_all,
+                            int32_t* seeded_all, float* cache, uint8_t* field, uint32_t* bits, int32_t* seeded, int store,
+                            ia_stream_t stream);
+
 /* Marching cubes (replaces skimage.measure.marching_cubes in utils/marching_cubes.py:29-30 and trimesh's
  * matrix_to_marching_cubes in DensityGrid.export_mesh, density_grid.py:112-116).  field [nx][ny][nz] fp32, x slowest;
  * nx, ny, nz >= 2 and 3*nx*ny*nz < 2^31, else IA_EINVAL (and the *_bytes queries return 0).  A lattice point is above

@@ -81,9 +81,13 @@ def save_checkpoint(model, path, epoch: int, loader=None):
                        "initial_lr": base[g], "params": ids})
     scheduler = {"base_lrs": base, "last_epoch": opt.epoch, "_step_count": opt.epoch + 1, "verbose": False,
                  "_get_lr_called_within_step": False, "_last_lr": [b * factor for b in base], "lr_lambdas": [None] * 3}
-    grids = [{"density_cached": _cpu(g.density_cached), "density_field": _cpu(g.density_field)}
-             | ({"bits": _cpu(g._bits)} if g._bits is not None else {})
-             for g in model.renderer.density_grid_train_all]
+    frames = _frame_grids(model)
+    if frames is not None:
+        grids = [{k: _cpu(v) for k, v in f.items()} for f in frames]
+    else:
+        grids = [{"density_cached": _cpu(g.density_cached), "density_field": _cpu(g.density_field)}
+                 | ({"bits": _cpu(g._bits)} if g._bits is not None else {})
+                 for g in model.renderer.density_grid_train_all]
     extra = {"grad_scaler": {"scale": _cpu(model.scaler.scale_t), "growth_tracker": _cpu(model.scaler.growth_tracker)},
              "adam_state": _cpu(opt.state_t), "train_grids": grids, "rng_cpu": torch.get_rng_state()}
     if model.pose_optimizer is not None:
@@ -102,6 +106,16 @@ def save_checkpoint(model, path, epoch: int, loader=None):
     tmp = path + ".tmp"
     torch.save(ckpt, tmp)
     os.replace(tmp, path)
+
+
+def _frame_grids(model):
+    """smpl_init: one dict of views per training frame into the stacked grids (cache, field, bits, seeded flag); else None"""
+    r = model.renderer
+    if not getattr(r, "smpl_init", False):
+        return None
+    fg = r.frame_grids
+    return [{"density_cached": fg.cache[f], "density_field": fg.field[f], "bits": fg.bits[f], "seeded": fg.seeded[f]}
+            for f in range(len(fg))]
 
 
 def _need(d, key, where):
@@ -176,14 +190,18 @@ def load_checkpoint(model, path, loader=None) -> dict:
     ignored = sorted(k for k in sd if k not in own)
     copies, steps = _plan_optimizer(model, opt_states[0])
     extra = ckpt.get(EXTRA_KEY)
-    grids = model.renderer.density_grid_train_all
+    frames = _frame_grids(model)
+    grids = model.renderer.density_grid_train_all if frames is None else frames
     if extra is not None:
         saved = _need(extra, "train_grids", EXTRA_KEY)
         if len(saved) != len(grids):
             raise ValueError(f"load_checkpoint: {len(saved)} train grids in the checkpoint, the model has {len(grids)}")
         for g, s in zip(grids, saved):
             for k in ("density_cached", "density_field"):
-                _same_shape(f"train grid {k}", _need(s, k, "a train grid"), getattr(g, k))
+                _same_shape(f"train grid {k}", _need(s, k, "a train grid"), g[k] if frames is not None else getattr(g, k))
+            for k in ("bits", "seeded") if frames is not None else ():
+                if k in s:
+                    _same_shape(f"train grid {k}", s[k], g[k])
         for k in ("grad_scaler", "adam_state"):
             _need(extra, k, EXTRA_KEY)
         if model.pose_optimizer is not None:
@@ -212,7 +230,13 @@ def load_checkpoint(model, path, loader=None) -> dict:
                 model.pose_optimizer.state_t.copy_(extra["pose_adam_state"])
             model.scaler.scale_t.copy_(extra["grad_scaler"]["scale"])
             model.scaler.growth_tracker.copy_(extra["grad_scaler"]["growth_tracker"])
-            for g, s in zip(grids, extra["train_grids"]):
+            if frames is not None:
+                # smpl_init: every frame's grid; a file without the seeded flags (or bits) leaves them as built
+                for g, s in zip(frames, extra["train_grids"]):
+                    for k in ("density_cached", "density_field", "bits", "seeded"):
+                        if k in s:
+                            g[k].copy_(s[k])
+            for g, s in zip(grids if frames is None else (), extra["train_grids"]):
                 g.density_cached.copy_(s["density_cached"])
                 g.density_field.copy_(s["density_field"])
                 g._version += 1

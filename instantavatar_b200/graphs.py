@@ -144,6 +144,9 @@ class GraphedTrainStep:
         ts.append(mlp_h)
         grid = m.renderer.density_grid_train
         ts += [grid.density_cached, grid.density_field] + ([grid._bits] if grid._bits is not None else [])
+        if getattr(m.renderer, "smpl_init", False):   # every frame's grid and seeded flag
+            fg = m.renderer.frame_grids
+            ts += [fg.cache, fg.field, fg.bits, fg.seeded, grid.seeded]
         if m.pose_optimizer is not None:
             ts += [p.data for p in m.pose_optimizer.params] + [t for mv in m.pose_optimizer.state for t in mv] + [m.pose_optimizer.state_t]
         return ts
@@ -157,6 +160,9 @@ class GraphedTrainStep:
         if "idx" not in self.static_in and model.SMPL_param is not None:
             raise ValueError("GraphedTrainStep with pose optimisation needs a static `idx` tensor in the batch "
                              "(a host scalar would become a pageable H2D copy inside the capture)")
+        if "idx" not in self.static_in and getattr(model.renderer, "smpl_init", False):
+            raise ValueError("GraphedTrainStep with smpl_init needs a static `idx` tensor in the batch (it selects the "
+                             "frame's occupancy grid on the device)")
         s = torch.cuda.Stream()
         s.wait_stream(torch.cuda.current_stream())
         with torch.cuda.stream(s):

@@ -199,8 +199,19 @@ class DNeRFModel(torch.nn.Module):
         self.frame_prepare(batch, jitters)
         return self.frame_render(batch, img_size)
 
-    def update_density_grid(self, jitter=None):
-        """DNeRF.py:99-110: every 20 steps refresh the train occupancy grid and return the density regulariser."""
+    def update_density_grid(self, jitter=None, frame=None):
+        """DNeRF.py:99-110: every 20 steps refresh the train occupancy grid and return the density regulariser.  With
+        smpl_init every step refreshes the grid of the step's frame (frame: device int64 [1], the batch's `idx`; required)."""
+        if getattr(self.renderer, "smpl_init", False):
+            if frame is None:
+                raise ValueError("update_density_grid: with smpl_init the step's frame index is required (frame: device "
+                                 "int64 [1], the batch's `idx`)")
+            density, valid = self.renderer.update_train_grid(self.deformer, self.net_coarse, self.global_step, frame, jitter)
+            inv = (~valid).float()
+            reg = (density * inv).sum() / inv.sum()  # N = 1: density[~valid].mean()
+            if self.global_step < 500:
+                reg = reg + 0.5 * density.mean()
+            return reg
         N = 20
         if self.global_step % N != 0:
             return None
@@ -225,9 +236,11 @@ class DNeRFModel(torch.nn.Module):
             idx = torch.as_tensor(batch.get("idx", 0), device=batch["rays_o"].device).reshape(-1)[:1].long()
             # steps whose only pose-dependent loss is the ray loss (all steps when refining, else those without the grid
             # regulariser) run without an autograd graph: ia_pose_grad -> ia_smpl_tfs_backward -> index_add_ into the
-            # embedding gradients; the whole step is then a fixed launch sequence (CUDA-graph capturable)
+            # embedding gradients; the whole step is then a fixed launch sequence (CUDA-graph capturable).  With
+            # smpl_init every step has the regulariser, whose density query depends on the pose (DNeRF.py:99-108, N = 1)
+            regularised = self.global_step % 20 == 0 or getattr(self.renderer, "smpl_init", False)
             manual_pose = (self.fused_loss and getattr(self.deformer, "fast_prepare", False)
-                           and (self.is_refine or self.global_step % 20 != 0))
+                           and (self.is_refine or not regularised))
             with torch.set_grad_enabled(not manual_pose):
                 body = self.SMPL_param(idx)
             # DNeRF.py:121-123: the nearest-vertex deformer also takes the (optimised) shape
@@ -242,7 +255,10 @@ class DNeRFModel(torch.nn.Module):
         self.deformer.prepare_deformer(batch)
         self.net_coarse.initialize(self.deformer.bbox)
         g_enc, g_col = self.net_coarse.grad_buffers()  # zeroed at creation and by every fused optimiser step
-        reg = self.update_density_grid(grid_jitter)
+        frame = None
+        if getattr(self.renderer, "smpl_init", False):   # the grid of the batch's frame, selected on the device (DNeRF.py:129)
+            frame = torch.as_tensor(batch.get("idx", 0), device=batch["rays_o"].device).reshape(-1)[:1].to(torch.int64)
+        reg = self.update_density_grid(grid_jitter, frame)
         if self.fused_loss:
             # forward kernel -> loss forward+backward kernel -> compositing backward -> network backward: no autograd
             # graph for the per-ray path (the grid regulariser below, and an LPIPS term, still go through autograd)

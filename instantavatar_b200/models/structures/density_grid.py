@@ -50,9 +50,14 @@ class DensityGrid(torch.nn.Module):
         self.register_buffer("density_field", torch.zeros_like(self.coords[..., 0], dtype=torch.bool))
         self.aabb = aabb
         self.initialized = False
-        if smpl_init:
-            raise NotImplementedError("smpl_init needs kaolin (reference demo.yaml only); out of scope, SURVEY.md §2.1 #3")
+        if smpl_init and torch.device(device).type != "cuda":
+            # the reference seeds these grids with kaolin's CUDA kernels; here ia_smpl_init_seed does: no CPU path
+            raise NotImplementedError("DensityGrid(smpl_init=True) seeds the grid from the SMPL mesh on the GPU; it needs a CUDA device")
         self.smpl_init = smpl_init
+        if smpl_init:
+            # the reference's `initialized` for this grid, on the device: the seeding kernel reads and sets it, so a step
+            # needs no host read and one CUDA graph serves seeded and unseeded frames
+            self.seeded = torch.zeros(1, device=device, dtype=torch.int32)
         self._bits = None
         self._bits_version = -1
         self._version = 0
@@ -98,11 +103,37 @@ class DensityGrid(torch.nn.Module):
             _, density = deformer(coords.reshape(-1, 3), net, eval_mode=False)
         density = density.clip(min=0).reshape(coords.shape[:-1])
         old = self.density_field.clone()
-        self.density_cached.copy_(torch.maximum(self.density_cached * 0.8, density.detach()))
-        self.build_from_density(self.density_cached)
+        if self.smpl_init and step < 500:
+            # density_grid.py:52-68: the first call seeds the field and cache from the posed mesh; later calls before
+            # step 500 leave both as they are
+            self.seed_from_mesh(deformer)
+        else:
+            self.density_cached.copy_(torch.maximum(self.density_cached * 0.8, density.detach()))
+            self.build_from_density(self.density_cached)
         density = 1 - torch.exp(0.01 * -F.relu(density))
         valid = self.density_field if step < 500 else old
         return density, valid
+
+    @torch.no_grad()
+    def seed_from_mesh(self, deformer):
+        """density_grid.py:54-68 unless this grid is seeded: field = distance to the posed SMPL mesh (deformer.vertices, root
+        frame; body_model.faces_tensor) below 0.01 or inside, at the cell centres; cache = max(0.8 cache, +inf there)"""
+        faces = deformer.body_model.faces_tensor
+        verts = deformer.vertices[0].detach().float().contiguous()
+        if getattr(self, "_faces_src", None) is not faces:
+            # checked once, when the int32 copy is made (the kernels index verts with these without a bound check)
+            if faces.dim() != 2 or faces.shape[1] != 3:
+                raise ValueError(f"smpl_init: faces must be [F, 3], got {tuple(faces.shape)}")
+            if faces.numel() and (int(faces.min()) < 0 or int(faces.max()) >= verts.shape[0]):
+                raise ValueError(f"smpl_init: face indices must lie in [0, {verts.shape[0]}), got "
+                                 f"[{int(faces.min())}, {int(faces.max())}]")
+            self._faces_src, self._faces = faces, faces.to(torch.int32).contiguous()
+        if self._bits is None:
+            self._bits = torch.empty(self.grid_size ** 3 // 32 + 8, device=verts.device, dtype=torch.int32)
+        self._seed_ws = ops.smpl_init_seed(verts, self._faces, self.aabb6(), self.grid_size, self.seeded, self.density_cached,
+                                           self.density_field, self._bits, getattr(self, "_seed_ws", None))
+        self._version += 1
+        self._bits_version = self._version
 
     @torch.no_grad()
     def initialize(self, deformer, net, iters=5, jitters=None, shard=(0, 1), peer=None):
@@ -148,3 +179,38 @@ class DensityGrid(torch.nn.Module):
         the occupied cells as a closed mesh in voxel-index units, meshed on the GPU (mesh.occupancy_surface)."""
         from ...mesh import occupancy_surface, to_mesh
         return to_mesh(*occupancy_surface(self.density_field))
+
+
+class FrameGrids:
+    """demo.yaml's per-frame train grids (raymarcher_acc.py:66-68 with smpl_init: one DensityGrid(64, aabb, smpl_init=True)
+    per training frame) in stacked device storage, plus one working DensityGrid that the training kernels read.  `load`
+    copies the grid of the frame a device index names into the working grid and `store` copies it back, so a step picks
+    its frame's grid without a host read."""
+
+    def __init__(self, n_frames: int, grid_size: int, aabb, device):
+        G = grid_size
+        self.working = DensityGrid(G, aabb, smpl_init=True, device=device)
+        self.working.occupancy_bits()   # the bit field of the empty grid: every frame starts from it
+        self.cache = torch.zeros((n_frames, G, G, G), device=device, dtype=torch.float32)
+        self.field = torch.zeros((n_frames, G, G, G), device=device, dtype=torch.bool)
+        self.bits = self.working._bits[None].repeat(n_frames, 1)
+        self.seeded = torch.zeros(n_frames, device=device, dtype=torch.int32)
+
+    def __len__(self):
+        return self.cache.shape[0]
+
+    def _copy(self, idx, store):
+        w = self.working
+        ops.occupancy_frame_copy(idx, self.cache, self.field, self.bits, self.seeded, w.density_cached, w.density_field,
+                                 w._bits, w.seeded, store)
+
+    def load(self, idx):
+        """working grid <- frame min(idx[0], N - 1); idx: device int64 [1]"""
+        self._copy(idx, False)
+        w = self.working
+        w._version += 1
+        w._bits_version = w._version
+
+    def store(self, idx):
+        """frame min(idx[0], N - 1) <- working grid"""
+        self._copy(idx, True)

@@ -84,6 +84,26 @@ def occupancy_build(density: torch.Tensor, bits=None, want_field=True, workspace
     return field, bits
 
 
+def smpl_init_seed(verts, faces_i32, aabb6, G: int, seeded, cache, field, bits, workspace=None):
+    """density_grid.py:52-68 (smpl_init, first step-< 500 update of a frame) unless seeded[0] != 0: field [G,G,G] bool =
+    distance to the mesh verts [V,3] / faces_i32 [F,3] below 0.01 or inside, cache [G,G,G] = max(0.8 cache, +inf where
+    occupied), bits = the packed field; then seeded[0] = 1.  -> the workspace (reuse it)."""
+    nbytes = call("ia_smpl_init_workspace_bytes", G)
+    if workspace is None or workspace.numel() < nbytes:
+        workspace = torch.empty(nbytes, device=verts.device, dtype=torch.uint8)
+    _lib.count(7 if faces_i32.shape[0] else 5)
+    call("ia_smpl_init_seed", verts, verts.shape[0], faces_i32, faces_i32.shape[0], aabb6, G, seeded, cache, field, bits,
+         workspace, workspace.numel(), STREAM)
+    return workspace
+
+
+def occupancy_frame_copy(idx, cache_all, field_all, bits_all, seeded_all, cache, field, bits, seeded, store: bool):
+    """frame clamp(idx[0], 0, N-1) of the stacked grids -> the working grid (store=False) or back (store=True)"""
+    N, G = cache_all.shape[0], cache_all.shape[1]
+    _lib.count(1); call("ia_occupancy_frame_copy", idx, N, G, cache_all, field_all, bits_all, seeded_all, cache, field, bits,
+                        seeded, int(store), STREAM)
+
+
 def mc_count(field: torch.Tensor, level: float, workspace=None):
     """marching cubes, first call: field [nx,ny,nz] fp32 -> (counts int64 [3] = n_verts, n_faces, n_nonfinite (device),
     workspace holding the classification and scans for mc_emit)"""

@@ -12,7 +12,7 @@ from __future__ import annotations
 import torch
 
 from .. import ops
-from ..models.structures.density_grid import DensityGrid
+from ..models.structures.density_grid import DensityGrid, FrameGrids
 
 
 class BoundModel:
@@ -50,11 +50,10 @@ class Raymarcher(torch.nn.Module):
         super().__init__()
         if MAX_SAMPLES != 256:
             raise ValueError("the fused kernels are built for MAX_SAMPLES = 256 (confs/renderer/raymarcher_acc.yaml)")
-        if smpl_init:
-            # demo.yaml: one DensityGrid(smpl_init=True) per training frame, voxelised from the SMPL mesh with kaolin
-            # (raymarcher_acc.py:57-66, density_grid.py:52-68) -- kaolin is absent; fail instead of silently training
-            # with the plain single-grid semantics
-            raise NotImplementedError("Raymarcher(smpl_init=True) needs kaolin (reference demo.yaml only); out of scope, DESIGN.md §8")
+        if smpl_init and torch.device(device).type != "cuda":
+            # demo.yaml: one DensityGrid(smpl_init=True) per training frame, seeded from the SMPL mesh on the GPU (the
+            # reference's kaolin calls, raymarcher_acc.py:57-66, density_grid.py:52-68): there is no CPU path
+            raise NotImplementedError("Raymarcher(smpl_init=True) seeds per-frame grids from the SMPL mesh on the GPU; it needs a CUDA device")
         self.MAX_SAMPLES = MAX_SAMPLES
         self.MAX_BATCH_SIZE = MAX_BATCH_SIZE
         self.aabb = torch.tensor([[-1.25, -1.55, -1.25], [1.25, 0.95, 1.25]]).float().to(device)
@@ -65,11 +64,25 @@ class Raymarcher(torch.nn.Module):
 
     def initialize(self, N):
         dev = self.aabb.device
+        if self.smpl_init:
+            # one grid per training frame (raymarcher_acc.py:66-68), stacked on the device; the working grid holds the
+            # step's frame (load_train_grid / store_train_grid)
+            self.frame_grids = FrameGrids(N, 64, self.aabb, dev)
+            self.density_grid_train_all = [self.frame_grids.working]
+            return
         self.density_grid_train_all = [DensityGrid(64, self.aabb, device=dev)]
 
     @property
     def density_grid_train(self):
         return self.density_grid_train_all[min(self.idx, len(self.density_grid_train_all) - 1)]
+
+    def update_train_grid(self, deformer, net, step, frame, jitter=None):
+        """smpl_init: DensityGrid.update on the grid of training frame min(frame[0], N - 1) (frame: device int64 [1]);
+        -> (density, valid) as DensityGrid.update returns them"""
+        self.frame_grids.load(frame)
+        density, valid = self.frame_grids.working.update(deformer, net, step, jitter)
+        self.frame_grids.store(frame)
+        return density, valid
 
     def __call__(self, rays, model, eval_mode=True, noise=0, bg_color=None):
         if eval_mode:
