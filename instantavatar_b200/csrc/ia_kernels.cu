@@ -94,7 +94,11 @@ struct FrameRay {
     int kbeg = 0, kend = -1;
 };
 
-// false (kbeg = 0, kend = -1) when no step of the ray can reach an occupied cell
+// false (kbeg = 0, kend = -1) when no step of the ray can reach an occupied cell.  The march's t_k is the sequential
+// float32 sum near + dt + dt + ..., which after k <= 1024 additions lies within 1024 * 2^-24 * max(|near|, |far|) of the
+// analytic near + k dt the step indices come from.  The margin is 2 steps plus that drift in steps (bounded by twice that,
+// 2^-13 max(|near|, |far|) / dt); the drift term is 0 unless far - near < max(|near|, |far|) / 32, so ordinary rays keep
+// the 2-step margin, and it grows to the whole march once t stalls.  The march stops at step 1023 (1024 steps).
 __device__ __forceinline__ bool load_ray(const RenderArgs& a, const FrameConst& fc, const int* __restrict__ cbox, int G, int ray,
                                          FrameRay& r) {
     r.ox = a.rays_o[ray * 3]; r.oy = a.rays_o[ray * 3 + 1]; r.oz = a.rays_o[ray * 3 + 2];
@@ -104,9 +108,11 @@ __device__ __forceinline__ bool load_ray(const RenderArgs& a, const FrameConst& 
     float t0, t1;
     occupied_interval(fc, cbox, G, r.ox, r.oy, r.oz, r.dx, r.dy, r.dz, t0, t1);
     if (!(cbox[6] != 0 && t0 <= t1 && r.dt > 0.f)) return false;
-    const float k0f = floorf((fmaxf(t0, r.t) - r.t) / r.dt) - 2.f, k1f = ceilf((fminf(t1, r.far) - r.t) / r.dt) + 2.f;
+    const float drift = fmaxf(fabsf(r.t), fabsf(r.far)) * 0x1p-13f;
+    const float margin = drift < r.dt ? 2.f : 2.f + floorf(drift / r.dt);  // no division on ordinary rays
+    const float k0f = floorf((fmaxf(t0, r.t) - r.t) / r.dt) - margin, k1f = ceilf((fminf(t1, r.far) - r.t) / r.dt) + margin;
     r.kbeg = (int)fminf(fmaxf(k0f, 0.f), 1024.f);
-    r.kend = (int)fminf(fmaxf(k1f, -1.f), 1024.f);
+    r.kend = (int)fminf(fmaxf(k1f, -1.f), 1023.f);
     return true;
 }
 
