@@ -406,6 +406,25 @@ int ia_vertex_skin_weights(const float* lbs_voxel, int D, int H, int W, const fl
                            const float* xc, int n, int K, uint8_t* joints, float* weights, float* dropped /*nullable*/,
                            int* n_fallback, ia_stream_t stream);
 
+/* Texture baking (DESIGN.md §3, "Texture baking"; the layout is csrc/ia_atlas.cuh's).  An atlas of size x size texels
+ * (x right, y down, row 0 on top) gives faces 2k and 2k+1 the square cell k of c = floor(size / n) texels, n =
+ * ceil(sqrt(ceil(n_faces / 2))) cells per row, at origin ((k mod n) c, (k div n) c); with L = c - 5, face 2k's corners
+ * are (1, 1), (1 + L, 1), (1, 1 + L) and face 2k+1's (c - 1, c - 1), (c - 1 - L, c - 1), (c - 1, c - 1 - L) in the cell.
+ * A texel belongs to face f when its centre lies within L-infinity distance 1 of f's triangle (at most one owner; all
+ * four bilinear taps of a point of the triangle are f's).
+ * ia_texture_atlas: layout = (n, c, L) of n_faces faces at `size`.  Host only, no GPU needed.
+ * ia_texture_points: over all texels (t = row * size + column): owner [size^2] int32 = the owning face or -1, points
+ *   [size^2][3] = b0 v0 + b1 v1 + b2 v2 in float32 for the barycentrics of the point of the face's flat triangle closest
+ *   (Euclidean, in texel space) to the texel centre (the centre itself inside the triangle; not moved onto any level set),
+ *   v_k = verts[faces[f][k]], and 0 for an unowned texel; uv [n_faces][3][2] (nullable) = the corners / size, glTF's
+ *   TEXCOORD_0 (OBJ's vt flips v: 1 - y / size).  faces [n_faces][3] int32 indices into verts [n_verts][3]: each in
+ *   [0, n_verts), the caller guarantees it (the kernel does not check).  n_faces = 0: nothing is done.
+ * Both: IA_EINVAL for size outside [64, 16384], n_faces < 0 (< 1 for ia_texture_atlas), c < 6 (the message names the
+ *   smallest size that fits) or a NULL pointer. */
+int ia_texture_atlas(int n_faces, int size, int layout[3]);
+int ia_texture_points(const float* verts, int n_verts, const int* faces, int n_faces, int size, int* owner, float* points,
+                      float* uv /*nullable*/, ia_stream_t stream);
+
 /* Pose gradient of the nearest-vertex deformer (scene->nv set).  For each of the first min(*count, capacity) list samples
  * of ia_composite_bwd with best >= 0: l_rz [capacity][3] holds (ray index, z, 0) -- what ia_composite_bwd writes into l_xd
  * when it is given the rays rays_o[i] = (i, 0, 0), rays_d[i] = (0, 1, 0) (z * 0 + i and z * 1 + 0 are exact).  The posed

@@ -8,6 +8,7 @@ callers use.
 """
 from __future__ import annotations
 
+import copy
 import os
 
 import numpy as np
@@ -20,11 +21,15 @@ EMPTY_MSG = "Surface level must be within volume data range."
 
 class Mesh:
     """vertices float64 [V,3] (the float32 kernel results widened, as trimesh stores them), faces int64 [F,3],
-    vertex_colors float32 [V,3] in [0, 1] or None"""
+    vertex_colors float32 [V,3] in [0, 1] or None; a textured mesh (bake_texture) also has uv float32 [F,3,2] (each face
+    corner's texture coordinate, glTF's convention: origin at the top left) and texture uint8 [S,S,3] (RGB, sRGB-encoded),
+    both None otherwise"""
 
     def __init__(self, vertices, faces, vertex_colors=None):
         self.vertices = np.asarray(vertices, dtype=np.float64).reshape(-1, 3)
         self.faces = np.asarray(faces, dtype=np.int64).reshape(-1, 3)
+        self.uv = None
+        self.texture = None
         self.vertex_colors = None
         if vertex_colors is not None:
             self.vertex_colors = np.asarray(vertex_colors, dtype=np.float32).reshape(-1, 3)
@@ -52,9 +57,13 @@ class Mesh:
 
     def export(self, path):
         """write `path` as binary little-endian PLY (.ply) or Wavefront OBJ (.obj); with vertex colours, PLY adds
-        uchar red / green / blue after x y z and OBJ writes `v x y z r g b`"""
+        uchar red / green / blue after x y z and OBJ writes `v x y z r g b`.  A textured OBJ also writes <stem>.mtl and
+        <stem>.png beside it, one `vt` per face corner (v flipped: 1 - y / S) and `f a/ta b/tb c/tc`; PLY has no standard
+        texture, so a textured mesh writes the same PLY as an untextured one."""
         ext = os.path.splitext(str(path))[1].lower()
         col = self.vertex_colors is not None
+        if self.texture is not None and ext == ".obj":
+            return self._export_textured_obj(str(path))
         if ext == ".ply":
             header = ("ply\nformat binary_little_endian 1.0\n"
                       f"element vertex {len(self.vertices)}\nproperty double x\nproperty double y\nproperty double z\n"
@@ -85,6 +94,43 @@ class Mesh:
                     f.write(f"f {a} {b} {c}\n")
         else:
             raise ValueError(f"unsupported mesh format {ext!r} (use .ply or .obj)")
+
+    def _export_textured_obj(self, path):
+        if self.uv is None or self.uv.shape != (len(self.faces), 3, 2):
+            raise ValueError("a textured mesh needs uv [F,3,2] for its texture")
+        stem = os.path.splitext(path)[0]
+        name = os.path.basename(stem)
+        with open(stem + ".png", "wb") as f:
+            f.write(encode_png(self.texture))
+        with open(stem + ".mtl", "w") as f:
+            f.write(f"newmtl {MATERIAL}\nKd 1 1 1\nmap_Kd {name}.png\n")
+        with open(path, "w") as f:
+            f.write(f"mtllib {name}.mtl\n")
+            if self.vertex_colors is not None:
+                for (x, y, z), (r, g, b) in zip(self.vertices.tolist(), self.vertex_colors.astype(np.float64).tolist()):
+                    f.write(f"v {x!r} {y!r} {z!r} {r!r} {g!r} {b!r}\n")
+            else:
+                for x, y, z in self.vertices.tolist():
+                    f.write(f"v {x!r} {y!r} {z!r}\n")
+            uv = self.uv.reshape(-1, 2).astype(np.float64)
+            for s_, t_ in zip(uv[:, 0].tolist(), (1.0 - uv[:, 1]).tolist()):
+                f.write(f"vt {s_!r} {t_!r}\n")
+            f.write(f"usemtl {MATERIAL}\n")
+            for i, (a, b, c) in enumerate((self.faces + 1).tolist()):
+                t = 3 * i + 1
+                f.write(f"f {a}/{t} {b}/{t + 1} {c}/{t + 2}\n")
+
+
+MATERIAL = "avatar"
+
+
+def encode_png(texture) -> bytes:
+    """an RGB uint8 image [H,W,3] as PNG bytes (cv2.imencode, which takes BGR)"""
+    import cv2
+    ok, buf = cv2.imencode(".png", np.ascontiguousarray(np.asarray(texture, np.uint8)[..., ::-1]))
+    if not ok:
+        raise RuntimeError("cv2.imencode could not encode the texture as PNG")
+    return buf.tobytes()
 
 
 def extract_surface(field: torch.Tensor, level, gradient_direction="ascent", div=1.0, ext=None, origin=None,
@@ -222,6 +268,42 @@ def avatar_mesh(deformer, net, resolution=256, *, level_set, space="canonical", 
     return to_mesh(verts, faces, rgb)
 
 
+TEXTURE_SIZE = 4096
+
+
+@torch.no_grad()
+def bake_texture(m: Mesh, deformer, net, size: int = TEXTURE_SIZE, space="canonical") -> Mesh:
+    """a copy of m with a per-face texture atlas baked from the network (DESIGN.md §3, "Texture baking"): uv [F,3,2] and
+    texture [size,size,3] uint8.  ia_texture_points maps every texel to its owning face and the point of that face's flat
+    triangle nearest the texel centre; the network's colour there (ia_ngp_forward canonical, ia_deform_query in eval
+    mode posed, as vertex_colors) is reversed from BGR to RGB and quantised by colors_u8's rule; unowned texels are 0.
+    `space` is the space m's vertices live in, as in avatar_mesh."""
+    if space not in SPACES:
+        raise ValueError(f"space must be 'canonical' or 'posed', got {space!r}")
+    if len(m.faces) == 0:
+        raise ValueError("bake_texture: the mesh has no faces")
+    if m.faces.min() < 0 or m.faces.max() >= len(m.vertices):
+        raise ValueError(f"faces: indices must lie in [0, {len(m.vertices)})")
+    size = int(size)
+    ops.texture_atlas(len(m.faces), size)     # refuses a size with no room for the faces before any GPU work
+    scene = _avatar_scene(deformer, net, space)
+    dev = net.encoder.params.device
+    verts = torch.from_numpy(m.vertices.astype(np.float32)).to(dev)
+    faces = torch.from_numpy(m.faces.astype(np.int32)).to(dev)
+    owner, points, uv = ops.texture_points(verts, faces, size)
+    owned = torch.nonzero(owner.reshape(-1) >= 0).squeeze(1)
+    pts = points.reshape(-1, 3)[owned]
+    rgb = torch.empty_like(pts)
+    for i, chunk in enumerate(pts.split(CHUNK)):
+        rgb[i * CHUNK:i * CHUNK + chunk.shape[0]] = _query(scene, space, chunk)[0]
+    texture = torch.zeros((size * size, 3), device=dev, dtype=torch.uint8)
+    texture[owned] = torch.round(rgb.flip(1).double().clamp(0.0, 1.0) * 255.0).to(torch.uint8)
+    out = copy.copy(m)
+    out.uv = uv.cpu().numpy()
+    out.texture = texture.reshape(size, size, 3).cpu().numpy()
+    return out
+
+
 def require_skinning_field(deformer):
     """refuse a deformer without a voxelised skinning field: TypeError for anything but a SNARFDeformer, RuntimeError
     before its prepare_deformer has run"""
@@ -253,7 +335,7 @@ def pose_tfs(deformer, poses) -> torch.Tensor:
 def skin_mesh(m: Mesh, deformer, poses) -> list:
     """a canonical mesh (avatar_mesh(..., space="canonical")) skinned into F poses by the avatar's own skinning field
     (ForwardDeformer.forward_skinning, deformer_torch.py:118-128) in one ia_skin_points launch: F Meshes in the SMPL root
-    frame of each pose (the frame of SNARFDeformer.vertices), sharing m's faces and colours"""
+    frame of each pose (the frame of SNARFDeformer.vertices), sharing m's faces, colours, UVs and texture"""
     tfs = pose_tfs(deformer, poses)
     fd = deformer.deformer
     xc = torch.from_numpy(m.vertices.astype(np.float32)).to(tfs.device)
@@ -262,6 +344,7 @@ def skin_mesh(m: Mesh, deformer, poses) -> list:
     for f in range(len(xd)):
         posed = Mesh(xd[f], m.faces)
         posed.faces, posed.vertex_colors = m.faces, m.vertex_colors
+        posed.uv, posed.texture = m.uv, m.texture
         out.append(posed)
     return out
 

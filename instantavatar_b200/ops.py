@@ -607,6 +607,31 @@ def vertex_skin_weights(lbs_voxel, offset_k, scale_k, xc, K: int = 4, want_dropp
     return (joints, weights, n_fallback, dropped) if want_dropped else (joints, weights, n_fallback)
 
 
+def texture_atlas(n_faces: int, size: int) -> tuple:
+    """(cells per row, cell size, leg) of the texture atlas of n_faces faces at size x size texels (ia_texture_atlas, host
+    only); ValueError with the library's message when there is no such atlas"""
+    layout = (C.c_int * 3)()
+    rc = _lib.lib().ia_texture_atlas(int(n_faces), int(size), layout)
+    if rc != 0:
+        raise ValueError(_lib.lib().ia_last_error().decode())
+    return tuple(layout)
+
+
+def texture_points(verts, faces_i32, size: int, want_uv=True):
+    """the atlas texels of faces_i32 [NF,3] (indices in [0, V), checked by the caller) on verts [V,3] (ia_texture_points;
+    DESIGN.md §3 "Texture baking") -> (owner int32 [S,S], points [S,S,3], uv [NF,3,2] with want_uv else None)"""
+    verts, faces_i32 = verts.reshape(-1, 3).contiguous(), faces_i32.reshape(-1, 3).contiguous()
+    NF, dev = faces_i32.shape[0], verts.device
+    if NF == 0:
+        raise ValueError("texture_points: the mesh has no faces")
+    owner = torch.empty((size, size), device=dev, dtype=torch.int32)
+    points = torch.empty((size, size, 3), device=dev, dtype=f32)
+    uv = torch.empty((NF, 3, 2), device=dev, dtype=f32) if want_uv else None
+    _lib.count(1 + want_uv)
+    call("ia_texture_points", verts, verts.shape[0], faces_i32, NF, size, owner, points, uv, STREAM)
+    return owner, points, uv
+
+
 _RAY_SLOT_CODES: dict = {}
 
 

@@ -24,6 +24,7 @@ SMPL_JOINT_NAMES = (
 _FLOAT, _UBYTE, _UINT = 5126, 5121, 5125
 _ARRAY_BUFFER, _ELEMENT_ARRAY_BUFFER = 34962, 34963
 _TRIANGLES = 4
+_LINEAR, _CLAMP_TO_EDGE = 9729, 33071
 _GLB_MAGIC, _GLB_JSON, _GLB_BIN = 0x46546C67, 0x4E4F534A, 0x004E4942
 
 
@@ -155,9 +156,8 @@ class _Buffer:
     def __init__(self):
         self.parts, self.size, self.views, self.accessors = [], 0, [], []
 
-    def add(self, a, gltf_type: str, component: int, target=None, bounds=False) -> int:
-        a = np.ascontiguousarray(a, {_FLOAT: "<f4", _UBYTE: "u1", _UINT: "<u4"}[component])
-        data = a.tobytes()
+    def add_view(self, data: bytes, target=None) -> int:
+        """a bufferView of raw bytes (an embedded image) -> its index"""
         view = {"buffer": 0, "byteOffset": self.size, "byteLength": len(data)}
         if target is not None:
             view["target"] = target
@@ -165,7 +165,12 @@ class _Buffer:
         pad = -len(data) % 4
         self.parts += [data, b"\0" * pad]
         self.size += len(data) + pad
-        width = {"SCALAR": 1, "VEC3": 3, "VEC4": 4, "MAT4": 16}[gltf_type]
+        return len(self.views) - 1
+
+    def add(self, a, gltf_type: str, component: int, target=None, bounds=False) -> int:
+        a = np.ascontiguousarray(a, {_FLOAT: "<f4", _UBYTE: "u1", _UINT: "<u4"}[component])
+        self.add_view(a.tobytes(), target)
+        width = {"SCALAR": 1, "VEC2": 2, "VEC3": 3, "VEC4": 4, "MAT4": 16}[gltf_type]
         acc = {"bufferView": len(self.views) - 1, "componentType": component, "count": a.size // width, "type": gltf_type}
         if bounds:
             flat = a.reshape(-1, width)
@@ -179,11 +184,15 @@ def _column_major(m) -> np.ndarray:
 
 
 def write_glb(path, positions, faces, skel: dict, joints, weights, normals=None, colors=None, rotations=None,
-              root_translation=None, fps: float = 30, world_rotation=None, name: str = "avatar"):
+              root_translation=None, fps: float = 30, world_rotation=None, name: str = "avatar", uv=None, texture_png=None):
     """one glTF 2.0 binary from arrays: positions [V,3], faces [NF,3] (counter-clockwise seen from outside), skel from
     skeleton_from_joints, joints [V,K] / weights [V,K] (K a multiple of 4, rows summing to 1), normals [V,3] and linear
     RGB colours [V,3] (optional), an animation from pose_tracks' rotations [F,24,4] and root_translation [F,3] (optional,
-    keyframe i at i / fps, LINEAR), and a fixed 3x3 world_rotation above the root joint (optional)."""
+    keyframe i at i / fps, LINEAR), and a fixed 3x3 world_rotation above the root joint (optional).
+    With uv [NF,3,2] (TEXCOORD_0 of each face corner) and texture_png (PNG bytes, sRGB) the mesh is written textured:
+    3 NF vertices, one per face corner, each with its source vertex's position, normal, joints and weights; indices
+    0 .. 3 NF - 1; one material whose base colour is the texture, sampled LINEAR / LINEAR with CLAMP_TO_EDGE and no
+    mipmaps (a per-face atlas bleeds across faces at coarser levels); no COLOR_0, which glTF would multiply in."""
     positions = np.asarray(positions, np.float32).reshape(-1, 3)
     V = len(positions)
     faces = np.asarray(faces).reshape(-1, 3)
@@ -193,12 +202,28 @@ def write_glb(path, positions, faces, skel: dict, joints, weights, normals=None,
         raise ValueError(f"joints and weights need the same multiple of 4 columns, got {joints.shape} and {weights.shape}")
     if faces.size and (faces.min() < 0 or faces.max() >= V):
         raise ValueError(f"faces: indices must lie in [0, {V})")
+    textured = uv is not None or texture_png is not None
+    if textured:
+        if uv is None or texture_png is None:
+            raise ValueError("a textured mesh needs both uv and texture_png")
+        if colors is not None:
+            raise ValueError("colors: a textured mesh has no COLOR_0 (glTF multiplies it into the base colour)")
+        uv = np.asarray(uv, np.float32)
+        if uv.shape != (len(faces), 3, 2):
+            raise ValueError(f"uv must be [{len(faces)},3,2], got {uv.shape}")
+        corner = faces.reshape(-1)
+        positions, joints, weights = positions[corner], joints[corner], weights[corner]
+        normals = None if normals is None else np.asarray(normals).reshape(V, 3)[corner]
+        V = len(corner)
+        faces = np.arange(V).reshape(-1, 3)
     buf = _Buffer()
     attrs = {"POSITION": buf.add(positions, "VEC3", _FLOAT, _ARRAY_BUFFER, bounds=True)}
     if normals is not None:
         attrs["NORMAL"] = buf.add(np.asarray(normals).reshape(V, 3), "VEC3", _FLOAT, _ARRAY_BUFFER)
     if colors is not None:
         attrs["COLOR_0"] = buf.add(np.asarray(colors).reshape(V, 3), "VEC3", _FLOAT, _ARRAY_BUFFER)
+    if textured:
+        attrs["TEXCOORD_0"] = buf.add(uv.reshape(V, 2), "VEC2", _FLOAT, _ARRAY_BUFFER)
     for n in range(K // 4):
         attrs[f"JOINTS_{n}"] = buf.add(joints[:, 4 * n:4 * n + 4], "VEC4", _UBYTE, _ARRAY_BUFFER)
         attrs[f"WEIGHTS_{n}"] = buf.add(weights[:, 4 * n:4 * n + 4], "VEC4", _FLOAT, _ARRAY_BUFFER)
@@ -242,6 +267,13 @@ def write_glb(path, positions, faces, skel: dict, joints, weights, normals=None,
         samplers.append({"input": times, "output": buf.add(root_translation, "VEC3", _FLOAT), "interpolation": "LINEAR"})
         channels.append({"sampler": 24, "target": {"node": 1, "path": "translation"}})
         doc["animations"] = [{"name": "poses", "samplers": samplers, "channels": channels}]
+    if textured:
+        doc["meshes"][0]["primitives"][0]["material"] = 0
+        doc["materials"] = [{"name": name, "pbrMetallicRoughness": {"baseColorTexture": {"index": 0}, "metallicFactor": 0,
+                                                                     "roughnessFactor": 1}}]
+        doc["textures"] = [{"sampler": 0, "source": 0}]
+        doc["samplers"] = [{"magFilter": _LINEAR, "minFilter": _LINEAR, "wrapS": _CLAMP_TO_EDGE, "wrapT": _CLAMP_TO_EDGE}]
+        doc["images"] = [{"bufferView": buf.add_view(bytes(texture_png)), "mimeType": "image/png"}]
     doc["buffers"] = [{"byteLength": buf.size}]
     doc["bufferViews"] = buf.views
     doc["accessors"] = buf.accessors
@@ -264,7 +296,8 @@ def export_glb(path, m, deformer, poses=None, fps: float = 30, influences: int =
     binary: the SMPL skeleton of its subject (skeleton), `influences` weights per vertex (rig_weights), normals from
     ia_vertex_normals, m's colours as linear RGB (the network's BGR reversed, sRGB decoded) and, with `poses` (a dict as
     skin_mesh takes), one animation whose skinned result at keyframe f is SMPL's world frame for pose f.  world_rotation:
-    a fixed 3x3 rotation above the root (diag(1, -1, -1) turns an OpenCV camera frame Y-up)."""
+    a fixed 3x3 rotation above the root (diag(1, -1, -1) turns an OpenCV camera frame Y-up).  A textured m (bake_texture)
+    is written with its UVs and its texture as an embedded PNG base-colour texture instead of vertex colours (write_glb)."""
     if influences not in ops.RIG_INFLUENCES:
         raise ValueError(f"influences must be one of {ops.RIG_INFLUENCES}, got {influences!r}")
     skel = skeleton(deformer)
@@ -274,6 +307,10 @@ def export_glb(path, m, deformer, poses=None, fps: float = 30, influences: int =
     verts = torch.from_numpy(m.vertices.astype(np.float32)).to(dev)
     faces = torch.from_numpy(m.faces.astype(np.int32)).to(dev)
     normals = ops.vertex_normals(verts, faces, ops.face_csr(m.faces, len(m.vertices), dev)).cpu().numpy()
+    if m.texture is not None:
+        from .mesh import encode_png
+        return write_glb(path, m.vertices, m.faces, skel, joints, weights, normals, None, tracks[0], tracks[1], fps,
+                         world_rotation, name, uv=m.uv, texture_png=encode_png(m.texture))
     colors = None if m.vertex_colors is None else srgb_to_linear(m.vertex_colors[:, ::-1])
     return write_glb(path, m.vertices, m.faces, skel, joints, weights, normals, colors, tracks[0], tracks[1], fps,
                      world_rotation, name)
